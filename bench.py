@@ -4,6 +4,7 @@
     python bench.py [--gpus N] [--steps K] [--warmup W]             # headline: C2, weak scaling
     python bench.py --workload {c1,c2,c3,c4,c5} [--scaling {weak,strong}] [...]
     python bench.py --impl reference [...]                          # the reference's CPU path
+    python bench.py --dump-outputs DIR [...]                        # also write the results as .npy
 
 Workloads (SURVEY §8d; inputs are the reference benchmarks' own, generated in HBM by
 b200_synthetic_generators_device):
@@ -21,9 +22,15 @@ N > 1 (torchrun, one process per GPU). weak: every rank owns a full-size generat
 The only exchange is an NCCL all-gather of one partial point per column and rank, then N-1 point
 additions (SURVEY §8e). c4 shards by column: no exchange at all.
 
-With no --workload the headline line (c2, weak) also carries an "extras" object: short runs of the
-other BASELINE configs at this N (N = 1: c3, the per-GPU shares of c4 and c5, pageable-memory e2e, the
-reference's own GPU kernels on the same inputs; N > 1: strong-scaling c2, c4, c5).
+--dump-outputs DIR writes, for every workload run, the commitments its last timed step returned:
+DIR/<workload>_device.npy (device-resident path) and DIR/<workload>_e2e.npy (host C ABI), one row per
+column, the specified bytes of the result as float32. The inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
+
+With no --workload the headline line (c2, weak) also carries an "extras" object: runs of the other
+BASELINE configs at this N with the same --steps and --warmup (N = 1: c3, the per-GPU shares of c4
+and c5, pageable-memory e2e, the reference's own GPU kernels on the same inputs; N > 1:
+strong-scaling c2, c4, c5).
 """
 import argparse
 import ctypes as C
@@ -58,7 +65,7 @@ def read_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
@@ -242,7 +249,25 @@ class Env:
         return tuple(float(x) for x in t)
 
 
-def run_workload(env, name, scaling, steps, warmup, with_e2e=True, sampler=None):
+def dump_outputs(dump_dir, name, curve, fixed, dev_result, e2e_result):
+    """The specified bytes of each commitment as float32. The fixed-base path returns projective points
+    whose coordinates depend on the order of additions, so they are normalised first (C oracle port)."""
+    k = res_bytes(curve, False)
+    os.makedirs(dump_dir, exist_ok=True)
+    for tag, r in (("device", dev_result), ("e2e", e2e_result)):
+        if r is not None:
+            r = np.ascontiguousarray(np.asarray(r)[:, :res_bytes(curve, fixed)])
+            if fixed:
+                from oracle import port
+                r = port.normalize(curve, r)
+            np.save(os.path.join(dump_dir, f"{name}_{tag}.npy"), r[:, :k].astype(np.float32))
+
+
+def res_bytes(curve, fixed):
+    return {0: 160, 1: 144, 2: 96, 3: 96}[curve] if fixed else {0: 32, 1: 48, 2: 65, 3: 65}[curve]
+
+
+def run_workload(env, name, scaling, steps, warmup, with_e2e=True, sampler=None, dump_dir=None):
     """Times one BASELINE workload at env.world GPUs. Returns a dict (rank 0) of measurements; every
     rank must call it."""
     torch, bb, dist, world, rank = env.torch, env.bb, env.dist, env.world, env.rank
@@ -372,11 +397,13 @@ def run_workload(env, name, scaling, steps, warmup, with_e2e=True, sampler=None)
         bb.synchronize()
         t_e2e = time.perf_counter() - t0
         env.barrier()
-        k = {0: 32, 1: 48, 2: 65, 3: 65}[curve]
+        k = res_bytes(curve, False)
         if not fixed:
             assert np.array_equal(np.asarray(e2e_result)[:, :k], dev_result[:, :k]), \
                 f"{name}: device-resident and end-to-end paths disagree"
     ms, t_e2e_m = env.max_over_ranks(ms, t_e2e or 0.0)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, name, curve, fixed, dev_result, e2e_result)
 
     res = {
         "workload": desc, "scaling": scaling, "n_per_gpu": n, "columns_per_gpu": ncol,
@@ -437,7 +464,8 @@ def run_cuda(args, rank, local_rank, world):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    main = run_workload(env, headline, scaling, args.steps, args.warmup)
+    dump = args.dump_outputs
+    main = run_workload(env, headline, scaling, args.steps, args.warmup, dump_dir=dump)
     clocks = sampler.stop() if rank == 0 else None
     st = release(main)
     curve = st["curve"]
@@ -452,7 +480,7 @@ def run_cuda(args, rank, local_rank, world):
                          "is serial"}
     if args.workload is None and not args.no_extras:
         # ---- the other BASELINE configs, short runs ------------------------------------------------
-        xs, xw = 5, 3
+        xs, xw = args.steps, args.warmup
         if world == 1:
             if headline == "c2" and rank == 0 and not args.no_cpu_baseline:
                 # same-config single-core reference MSM on the bench's own inputs: the CPU number at
@@ -489,7 +517,7 @@ def run_cuda(args, rank, local_rank, world):
                         best = min(best, (whole, kern))
                     extras["refgpu"] = {"kernels_ms": best[1], "with_copies_ms": best[0],
                                         "what": "the reference's own bucket-method CUDA kernels compiled "
-                                                "for sm_100a (oracle/_ref/libblitzar_ref_gpu.so), same "
+                                                "for sm_90a (oracle/_ref/libblitzar_ref_gpu.so), same "
                                                 "C2 inputs, same GPU; kernels only, not its host pipeline"}
             del st
             for nm in ("c3", "c4_share", "c5_share", "c1"):
@@ -497,7 +525,7 @@ def run_cuda(args, rank, local_rank, world):
                     WORKLOADS[nm] = (0, 20, 8, 52, 0x0F, "C4 per-GPU share: 8 columns x n=2^20 ristretto255")
                 if nm == "c5_share":
                     WORKLOADS[nm] = (2, 21, 1, 96, 0x3F, "C5 per-GPU share: bn254 fixed-base MSM, n=2^21")
-                r = run_workload(env, nm, "strong", xs, xw)
+                r = run_workload(env, nm, "strong", xs, xw, dump_dir=dump)
                 s2 = release(r)
                 if rank == 0 and nm in ("c3", "c5_share"):
                     s2["fixed"] = nm == "c5_share"
@@ -506,14 +534,14 @@ def run_cuda(args, rank, local_rank, world):
                 extras[nm] = r
         else:
             del st
-            r = run_workload(env, "c2", "strong", xs, xw)
+            r = run_workload(env, "c2", "strong", xs, xw, dump_dir=dump and os.path.join(dump, "strong"))
             release(r)
             extras["c2_strong"] = r
             if 64 % world == 0:
-                r = run_workload(env, "c4", "strong", xs, xw)
+                r = run_workload(env, "c4", "strong", xs, xw, dump_dir=dump)
                 release(r)
                 extras["c4"] = r
-            r = run_workload(env, "c5", "strong", xs, xw)
+            r = run_workload(env, "c5", "strong", xs, xw, dump_dir=dump)
             release(r)
             extras["c5"] = r
 
@@ -524,14 +552,6 @@ def run_cuda(args, rank, local_rank, world):
                             "per term); see DESIGN.md")
             roof["secondary"] = imad_roofline(main["n_per_gpu"], roof["kernel_ms"] * roof["launches_per_step"],
                                               clocks)
-            prof = os.path.join(ROOT, "profiles", "r02_accumulate_traffic.json")
-            if os.path.exists(prof):
-                try:
-                    j = json.load(open(prof))
-                    roof["traffic"] = j.get("dram_bytes_per_launch")
-                    roof["traffic_source"] = "profiles/r02_accumulate_traffic.json (ncu --set full capture)"
-                except Exception:
-                    pass
         line = {
             "metric": METRIC if headline == "c2" else "MSM throughput (terms/s), " + main["workload"],
             "value": main["value"], "unit": "terms/s", "n_gpus": world,
@@ -541,7 +561,7 @@ def run_cuda(args, rank, local_rank, world):
             "config": {"workload": main["workload"] + (" per GPU (generator-range shard per rank)"
                                                        if main["scaling"] == "weak" else ""),
                        "global_terms": main["global_terms"], "curve": KERNEL_NAMES[curve],
-                       "cache": "inputs per step exceed the 126 MB L2",
+                       "cache": "inputs per step exceed the 50 MB L2",
                        "parallelism": f"generator-range x{world}" if headline != "c4" else f"columns x{world}"},
             "e2e": main.get("e2e"),
             "gpu_launches": main["gpu_launches"],
@@ -562,15 +582,16 @@ def imad_roofline(n, kernel_ms, clocks):
     """The bound that actually limits the accumulation kernel: the 32x32->64 multiplier. One term
     has 16 signed 16-bit digits (252-bit scalars), i.e. 16 bucket entries; every entry except the
     first of a bucket run is one cached-form addition = 8 field multiplications = 8 x (64 + 8)
-    IMAD.WIDE.U32 (schoolbook 8x8 limbs + the 2^256 = 38 fold). Peak = 29.2 lane-ops/clk/SM measured
-    on B200 for the multiply-accumulate-with-carry form this kernel issues (tests/micro/pipes.cu;
-    plain IMAD.WIDE 23.0, IMAD.HI 24.6) x 148 SMs x the SM clock sampled during the run."""
+    IMAD.WIDE.U32 (schoolbook 8x8 limbs + the 2^256 = 38 fold). Peak = 31.9 lane-ops/clk/SM measured
+    on an H100 SXM (700 W limit) for the multiply-accumulate-with-carry form this kernel issues
+    (tests/micro/pipes.cu; plain IMAD.WIDE 23.1, IMAD.HI 24.4) x 132 SMs x the SM clock sampled
+    during the run."""
     windows, nbuckets = 16, 1 << 15
     entries = windows * n * (1.0 - 2.0 ** -16)  # zero digits are skipped
     runs = windows * nbuckets * (1.0 - (1.0 - 1.0 / nbuckets) ** (entries / windows))
     imads = (entries - runs) * 8 * 72
-    mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    peak = 29.2 * 148 * mhz * 1e6
+    mhz = (clocks or {}).get("sm_mhz") or 1980.0
+    peak = 31.9 * 132 * mhz * 1e6
     achieved = imads / (kernel_ms * 1e-3)
     return {"bound": "imad_wide", "achieved": achieved, "peak": peak, "unit": "IMAD.WIDE lane-ops/s",
             "frac": achieved / peak, "imad_wide_per_step": imads}
@@ -586,6 +607,8 @@ def main():
     ap.add_argument("--scaling", default=None, choices=["weak", "strong"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write each workload's last-step results to DIR/<workload>_{device,e2e}.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,6 +1,6 @@
-"""Builds the in-tree native artefacts (no JIT cache): the product CUDA library for sm_100a, and —
-as test infrastructure — the CPU emulation harness, the C oracle port and, when /root/reference
-is present, the reference's own CPU path (oracle/_ref)."""
+"""Builds the in-tree native artefacts (no JIT cache): the product CUDA library for sm_90a (H100), and
+— as test infrastructure — the CPU emulation harness, the C oracle port and, when BLITZAR_REFERENCE
+names a checkout of the reference, the reference's own CPU and GPU paths (oracle/_ref)."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,8 @@ CSRC = os.path.join(ROOT, "blitzar_b200", "csrc")
 LIBDIR = os.path.join(ROOT, "blitzar_b200", "lib")
 LIB = os.path.join(LIBDIR, "libblitzar_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-std=c++17", "-O3"] + ARCH + ["-lineinfo",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC"]
 UNITS = ["api.cu", "curve_ed25519.cu", "curve_bls12381.cu", "curve_bn254.cu", "curve_grumpkin.cu"]
 
@@ -36,7 +37,7 @@ def build_product(verbose=False):
         src = os.path.join(CSRC, u)
         obj = os.path.join(LIBDIR, u.replace(".cu", ".o"))
         objs.append(obj)
-        if _newer(obj, [src] + _headers()):
+        if _newer(obj, [src, os.path.abspath(__file__)] + _headers()):
             cmd = [NVCC] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", src, "-o", obj]
             procs.append((u, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
     for u, p in procs:
@@ -46,7 +47,7 @@ def build_product(verbose=False):
         if p.returncode:
             raise RuntimeError(f"nvcc failed for {u}")
     if procs or not os.path.exists(LIB):
-        subprocess.check_call([NVCC, "-shared", "-o", LIB] + objs +
+        subprocess.check_call([NVCC, "-shared"] + ARCH + ["-o", LIB] + objs +
                               ["-Xlinker", "--version-script=" + os.path.join(CSRC, "export.map")])
     return LIB
 
@@ -87,12 +88,13 @@ def build_oracle_port():
 
 
 def build_oracle_ref():
-    """Only possible where /root/reference exists (this container); the GPU box uses the prebuilt
-    oracle/_ref/libblitzar_ref_cpu.so that travels with the snapshot."""
-    if not os.path.isdir("/root/reference/sxt"):
+    """Only where BLITZAR_REFERENCE names a checkout of the reference (spaceandtimefdn/blitzar).
+    Without it the tests compare against the reference results recorded under tests/golden/."""
+    ref = os.environ.get("BLITZAR_REFERENCE")
+    if not ref or not os.path.isdir(os.path.join(ref, "sxt")):
         return None
-    subprocess.check_call(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "ref_build")],
-                          stdout=subprocess.DEVNULL)
+    subprocess.check_call(["make", "-s", "-j8", "-C", os.path.join(ROOT, "oracle", "ref_build"),
+                           "R=" + os.path.abspath(ref)], stdout=subprocess.DEVNULL)
     return os.path.join(ROOT, "oracle", "_ref", "libblitzar_ref_cpu.so")
 
 

@@ -111,7 +111,7 @@ void ensure_device() {
 }
 
 // Window width of a fixed-base table over n generators of a curve on the current device: at most
-// 40 % of the free HBM (180 GB per B200: n = 2^24 bn254 generators take 14 GB at c = 20), overridable
+// 40 % of the free HBM (80 GB per H100: n = 2^24 bn254 generators take 14 GB at c = 20), overridable
 // with BLITZAR_B200_TABLE_WINDOW (0 disables tables).
 unsigned choose_table_window(uint64_t n, size_t gen_bytes) {
   if (const char* env = std::getenv("BLITZAR_B200_TABLE_WINDOW")) {
@@ -166,7 +166,7 @@ const CurveVTable& vt(unsigned curve_id) {
 
 
 // Host-to-device upload of PAGEABLE caller memory. A plain cudaMemcpyAsync from pageable memory is
-// staged by the driver on one thread (~8-10 GB/s measured: 192 MiB took ~20 ms of a 23 ms call).
+// staged by the driver on one thread, at the copy rate of one core.
 // Here a small persistent thread pool copies 8 MiB chunks into a ring of pinned buffers in parallel
 // while the previous chunk is in flight on the copy stream. Pinned caller memory (as bench.py
 // passes) goes straight to cudaMemcpyAsync.
@@ -207,11 +207,11 @@ public:
 private:
   static constexpr size_t kChunk = 8u << 20;
   static constexpr int kSlots = 4;
-  // threads copying one chunk into the pinned ring (the caller's included); a B200 host has on the
-  // order of 100 cores and one core moves ~10 GB/s, PCIe 5 x16 wants ~55 GB/s
+  // threads copying one chunk into the pinned ring (the caller's included); one core moves ~10 GB/s,
+  // PCIe 5 x16 wants ~55 GB/s
   const int kWorkers = [] {
     const char* env = std::getenv("BLITZAR_B200_STAGER_THREADS");
-    const int v = env ? std::atoi(env) : 4;  // measured on the B200 host: 2: 16.0, 4: 8.0, 8: 12.4, 16: 9.2 ms (n = 2^20)
+    const int v = env ? std::atoi(env) : 4;  // tests/e2e_pageable.py; RESULTS.md §4
     return std::max(1, std::min(32, v));
   }();
   unsigned char* staging_[kSlots] = {};
@@ -360,24 +360,23 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
   }
   // Upload in pieces so that sorting / accumulating piece r overlaps the PCIe copy of piece r+1
   // (later pieces accumulate into a scratch bucket array and are merged, MergeBucketsBody). Measured
-  // on B200 through this call, pinned inputs, ristretto (tests/e2e_ranges.py), ms for 1/2/4/8 pieces:
-  //   1 column : n=2^18 2.60/2.51/3.10/3.96  2^20 6.80/5.87/5.51/6.88  2^22 23.7/20.1/17.8/16.8
-  //   4 columns: n=2^19 8.31/7.61/8.21/9.82  2^20 15.2/13.3/13.4/15.2  2^22 54.6/45.0/42.1/42.6
-  // every piece costs ~0.3 ms of fixed sort / cascade work, hence pieces of >= 2^18 terms.
+  // on an H100 SXM through this call, pinned inputs, ristretto (tests/e2e_ranges.py), ms for 1/2/4/8
+  // pieces: 1 column n=2^20 7.45/6.07/5.56/6.18, 4 columns n=2^20 19.0/16.5/15.9 (1/2/4).
+  // Every piece costs fixed sort / cascade work, hence pieces of >= 2^18 terms.
   uint32_t num_ranges = (uint32_t)std::min<uint64_t>(n >> 18, num == 1 ? 8 : 4);
   if (num == 1 && n >= (1ull << 18))
     num_ranges = std::max(num_ranges, 2u);
   // the Weierstrass curves pay a fixed cost per piece and batch-affine level (inversion trees, scratch
-  // bucket merge): pieces of >= 2^21 terms. bls12-381 n = 2^22 from pinned memory, 1 / 2 / 3 / 4 / 8
-  // pieces: 42.4 / 41.4 / 46.1 / 46.3 / 52.0 ms (tests/e2e_c3_ranges.py)
+  // bucket merge): pieces of >= 2^21 terms. bls12-381 n = 2^22 from pinned memory on an H100 SXM,
+  // 1 / 2 / 3 / 4 / 8 pieces: 55.0 / 53.4 / 57.3 / 56.2 / 58.3 ms (tests/e2e_c3_ranges.py)
   if (curve_id != SXT_CURVE_RISTRETTO255)
     num_ranges = (uint32_t)std::min<uint64_t>(n >> 21, 4);
   num_ranges = std::max(num_ranges, 1u);
   if (const char* env = std::getenv("BLITZAR_B200_RANGES"))
     num_ranges = (uint32_t)std::max(1, std::min(16, std::atoi(env)));
   // piece schedule: equal pieces. Shrinking pieces (less work after the last byte of an upload-bound
-  // call) and growing pieces (earlier first kernel of a compute-bound call) were measured and lose:
-  // C2 e2e 5.22 -> 5.62 ms, C3 39.3 -> 39.7 ms (BLITZAR_B200_RANGE_SKEW = 1 / -1 selects them)
+  // call) and growing pieces (earlier first kernel of a compute-bound call) lose on an H100: C2 e2e
+  // 6.81 / 6.15 ms against 5.86, C3 58.0 / 54.6 ms against 54.3 (BLITZAR_B200_RANGE_SKEW = 1 / -1)
   int skew = 0;
   if (const char* env = std::getenv("BLITZAR_B200_RANGE_SKEW"))
     skew = std::atoi(env);
@@ -822,7 +821,11 @@ int sxt_init(const struct sxt_config* config) {
   if (const char* env = std::getenv("BLITZAR_B200_DEVICES")) {
     int want = std::atoi(env), count = 0;
     B200_CUDA(cudaGetDeviceCount(&count));
-    want = std::min(want, count);
+    // test hook: BLITZAR_B200_SHARED_DEVICES=1 lets the k shards share fewer devices (round-robin,
+    // separate streams and state), so the sharded paths can be tested on one GPU
+    const char* shared = std::getenv("BLITZAR_B200_SHARED_DEVICES");
+    if (!(shared && std::atoi(shared) != 0))
+      want = std::min(want, count);
     for (int k = 1; k < want; ++k) {
       auto w = std::make_unique<Worker>((g_state.device + k) % count);
       Worker* wp = w.get();

@@ -29,8 +29,8 @@ constexpr u32 kPadIndex = 0x7fffffffu;  // generator index of a pad entry (ident
 constexpr u32 kBatchGroup = 8;          // arity of the inversion tree: short serial chains per thread, the
                                         // levels above the first are latency-bound either way
 constexpr u32 kBatchTop = 4;            // at most this many values reach the top of the tree (their
-                                        // data-dependent inversions diverge within a warp: 64 lanes took
-                                        // 303 us for bls12-381 against ~100 us for a handful)
+                                        // data-dependent inversions diverge within a warp: 64 lanes take
+                                        // several times as long as a handful)
 
 // ---- in-place batch inversion of n non-zero field elements ----------------------------------------
 template <class F> struct BatchUpBody {

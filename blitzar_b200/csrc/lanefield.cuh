@@ -14,8 +14,8 @@
 //
 // (A first version kept the saturated 8 x 32-bit limbs of field.cuh across 8 lanes and resolved
 // the carries exactly with a ballot-based carry-lookahead; its dependent chain — two ballots and
-// two resolutions per operation — made it no faster than the quad-lane schedule: 272 vs 274 us for
-// the C2 Horner kernel.)
+// two resolutions per operation — made it no faster than the quad-lane schedule for the C2 Horner
+// kernel.)
 //
 // Replaces, for these chains, the per-thread schedules of field.cuh (which replace
 // sxt/field51/operation/{mul,sq}.cc). Device only: the CPU emulation harness keeps the scalar path.

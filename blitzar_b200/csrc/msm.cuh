@@ -9,13 +9,13 @@
 // multiproduct_gpu/kernel.h). One algorithm covers every input shape the ABI admits:
 // 1..32-byte unsigned, power-of-two signed, ragged lengths, bit-packed and strided scalar tables.
 //
-// Design (B200-first, not the reference's): the reference gives one thread a 1/192 slice of the
+// Design (GPU-first, not the reference's): the reference gives one thread a 1/192 slice of the
 // terms and read-modify-writes 255 global-memory buckets per window with c = 8; here every term is
 // decomposed into signed c-bit digits (c up to 16, chosen from n), the (window,bucket) keys are
 // counting-sorted so each bucket is a contiguous run of generator indices, and the runs are
 // summed by a load-balanced chunk walk (every thread sums exactly K consecutive sorted entries,
 // whatever the bucket-size distribution) followed by a short cascade over chunk-boundary pieces.
-// Bucket arrays live in HBM once per window (no per-block replicas), sized for 180 GB.
+// Bucket arrays live in HBM once per window (no per-block replicas), capped at kMaxBucketBytes.
 //
 // Round 2: the short Weierstrass curves run the first levels of the bucket sums as batch-affine pair
 // additions (batch_affine.cuh) before the chunk walk; fixed-base calls run in table mode (all windows of
@@ -309,7 +309,7 @@ template <class C> struct FillIdentityBody {
 // buckets[k] += scratch[k] for every bucket the current generator range touched (bucket_end = the
 // range's cursor array after the scatter). A later range accumulates into its own scratch array and
 // is merged here: one coalesced pass, instead of a read-add-write at every run boundary of the
-// accumulation kernel (measured on B200, C2 in 4 pieces: 1.05 ms per piece that way vs 0.47 ms).
+// accumulation kernel (about twice as fast per piece at C2 in 4 pieces).
 template <class C> struct MergeBucketsBody {
   static constexpr int kBlock = 128;
   const u32* bucket_end;
@@ -797,8 +797,7 @@ template <class C> struct SumPartsBody {
 // ---- host orchestration --------------------------------------------------------------------------
 // c minimising (windows) x (terms + bucket-reduction work), with the bucket arrays of all columns
 // capped at kMaxBucketBytes of HBM. Widths up to 20 are supported (b200_set_tuning) but the automatic
-// choice stops at 16: measured on B200 at n = 2^24, c = 20 saves 3.2 ms of accumulation and costs
-// 5.9 ms of extra bucket reduction (34.8 ms at c = 16 vs 37.4 ms).
+// choice stops at 16: at n = 2^24, c = 20 saves less accumulation than it adds bucket reduction.
 inline u32 choose_window_bits(u64 max_n, u32 max_width, u32 ncols, size_t point_bytes) {
   const double kMaxBucketBytes = 3.0e9;
   u32 best = 2;
@@ -917,8 +916,8 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
     if (opt.pair_levels >= 0)
       L = (u32)opt.pair_levels;
     else if (max_entries >= (1ull << 23))  // below ~2^19 terms the per-level fixed costs lose (measured)
-      while (L < 6 && (double)(32u << L) <= mean)  // measured on B200: 2 levels at a mean load of 64,
-        ++L;                                        // 3 at 128 (tests/pair_timing.py)
+      while (L < 6 && (double)(32u << L) <= mean)  // 2 levels at a mean load of 64, 3 at 128
+        ++L;                                        // (tests/pair_timing.py)
     while (L > 0 && max_entries + nkeys * ((1ull << L) - 1) >= (1ull << 32) - (1ull << L))
       --L;
   }
@@ -1034,7 +1033,7 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
   }
 
   // a chunk of K entries leaves 2 pieces, so K must exceed 2 for the cascade to shrink
-  // measured on B200 (C2): K = 64 trims the cascade more than it costs the first level
+  // at C2, K = 64 trims the cascade more than it costs the first level
   const u32 chunk1_auto = m_max >= (1ull << 23) ? 64u : 32u;
   const u32 chunk1 = opt.chunk1 == 0 ? chunk1_auto : (opt.chunk1 < 4 ? 4u : opt.chunk1);
   const u32 chunkn = opt.chunkn < 4 ? 4u : opt.chunkn;
@@ -1062,8 +1061,8 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
     const u32 fin = final_level ? 1u : 0u;
     if (first) {
       const u32 unit_z = (walk_gens == gens && opt.gens_normalized) ? 1u : 0u;
-      // measured on B200: ed25519 C2 2.894 -> 2.764 ms (a run start is a multiplication by a constant
-      // there); the Weierstrass start is free, so the extra addition loses (bn254 10.71 -> 10.94 ms)
+      // faster on ed25519 (a run start is a multiplication by a constant there); the Weierstrass
+      // start is free, so the extra addition loses
       const bool uniform =
           opt.uniform_add == 2 ? C::kCurveId == kRistretto255 : opt.uniform_add != 0;
       if (uniform)

@@ -1,7 +1,7 @@
 /* The reference's C example (example/cbindings1/main.cc: three rows of three 1-byte scalars committed
  * over the built-in generators), written against include/blitzar_b200.h in plain C99. It also shows the
  * fixed-generator handle API. Build: gcc -std=c99 -Iinclude examples/cbindings1.c -Lblitzar_b200/lib
- * -lblitzar_b200 -o cbindings1   (run on a machine with a B200; the library has no CPU fallback). */
+ * -lblitzar_b200 -o cbindings1   (run on a machine with an H100; the library has no CPU fallback). */
 #include <stdio.h>
 #include <string.h>
 

@@ -1,4 +1,4 @@
-/* blitzar_b200 — C ABI of the B200-native MSM / Pedersen-commitment backend.
+/* blitzar_b200 — C ABI of the H100-native (sm_90a) MSM / Pedersen-commitment backend.
  *
  * Part 1 ("sxt_*") is the drop-in boundary: the same 18 symbols, struct layouts and argument
  * meaning as the reference's cbindings/blitzar_api.h (line numbers of the reference declaration

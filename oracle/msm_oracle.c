@@ -5,7 +5,7 @@
  *
  * Parity is PINNED: this file is checked (tests/test_oracle.py) against
  *   - the reference's own golden commitments (rust/tests/src/main.rs:30-49), and
- *   - the reference's own CPU implementation compiled from /root/reference (oracle/_ref), on
+ *   - the reference's own CPU implementation compiled from a reference checkout (oracle/_ref), on
  *     random inputs for all four curves, both APIs, and committed fixtures (tests/golden/).
  *
  * What is restated (reference file:line):

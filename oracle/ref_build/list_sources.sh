@@ -1,6 +1,6 @@
 #!/bin/bash
 # Lists the reference translation units the CPU MSM path needs (SURVEY.md Appendix A).
-R=${1:-/root/reference}
+R=${1:?usage: list_sources.sh <reference checkout>}
 find $R/sxt/base/{bit,container,error,num,memory,iterator,type,field,curve,functional,device,macro} \
      $R/sxt/memory $R/sxt/execution/{async,device,schedule,kernel} \
      $R/sxt/{field51,curve21,ristretto,scalar25,field12,curve_g1,field25,curve_bng1,fieldgk,curve_gk} \

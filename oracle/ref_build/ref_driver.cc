@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — not product code.
 //
 // Thin C-ABI driver over the UNMODIFIED reference cpu-backend sources (compiled where they lie under
-// /root/reference by oracle/ref_build/Makefile; outputs go to oracle/_ref/ only). It exposes the
+// a reference checkout by oracle/ref_build/Makefile; outputs go to oracle/_ref/ only). It exposes the
 // reference's own CPU implementation of the MSM hot path as `ref_*` symbols so tests and
 // bench.py's cpu_baseline / `--impl reference` leg can call it through ctypes.
 //

@@ -2,7 +2,7 @@
 //
 // Stand-in for the reference's GPU backend on the C2 path: its own bucket-method kernels
 // (sxt/multiexp/bucket_method/accumulation_kernel.h:38, combination_kernel.h:40,81), compiled
-// unmodified for sm_100a from /root/reference, launched with the geometry of
+// unmodified for sm_90a from the reference checkout, launched with the geometry of
 // accumulation.h:54-95 and multiexponentiation.h:55-86 (one output, one device, whole range), then
 // the host combine_buckets of combination.h:50-62. It covers the reference's KERNELS and copies
 // only — not its coroutine scheduler, chunking or multi-device split, which nvcc cannot build
@@ -34,6 +34,13 @@ using E = c21t::element_p3;
     }                                                                                              \
   } while (0)
 
+// 0 when the kernels have an image for the current device: a library built for another architecture
+// loads, but its launches fail.
+extern "C" int ref_gpu_probe() {
+  cudaFuncAttributes a;
+  return (int)cudaFuncGetAttributes(&a, mtxbk::bucket_accumulate<E>);
+}
+
 // generators: n x 160 B (host), scalars: n x 32 B (host), out: one element_p3 (160 B).
 // times_ms[0] = whole call (H2D + kernels + D2H + host combine, wall clock of the GPU part by events),
 // times_ms[1] = the three kernels only.
@@ -63,6 +70,7 @@ extern "C" int ref_gpu_bucket_msm(void* out, const void* generators, const uint8
       <<<dim3(kGroupSize, 1, 1), kGroups>>>(d_sums, d_partial, num_blocks);
   mtxbk::combine_bucket_groups<kGroupSize, kGroups, E>
       <<<dim3((kGroupSize + 31) / 32, 1, 1), 32>>>(d_reduced, d_sums);
+  CK(cudaGetLastError());
   CK(cudaEventRecord(e2));
   CK(cudaMemcpyAsync(reduced.data(), d_reduced, sizeof(E) * kGroupSize, cudaMemcpyDeviceToHost));
   CK(cudaEventRecord(e3));

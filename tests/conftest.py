@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -21,12 +21,31 @@ def port():
 
 
 @pytest.fixture(scope="session")
-def refcpu():
-    """The reference's own CPU path (oracle/_ref), when the prebuilt library is present."""
+def _reference_store():
+    from tests import recorded_reference as rr
+    store = rr.Store()
+    yield store
+    if os.environ.get("BLITZAR_RECORD_REFERENCE"):
+        store.save(os.environ["BLITZAR_RECORD_REFERENCE"])
+
+
+def _reference(store, label, module):
+    from tests import recorded_reference as rr
+    return rr.RecordedReference(label, module if module.available() else None, store)
+
+
+@pytest.fixture(scope="session")
+def refcpu(_reference_store):
+    """The reference's own CPU path (oracle/_ref) when built, else its recorded answers."""
     from oracle import refcpu as r
-    if not r.available():
-        pytest.skip("oracle/_ref/libblitzar_ref_cpu.so not built")
-    return r
+    return _reference(_reference_store, "refcpu", r)
+
+
+@pytest.fixture(scope="session")
+def refgpu(_reference_store):
+    """The reference's own GPU bucket kernels (oracle/_ref) when built, else their recorded answers."""
+    from oracle import refgpu as r
+    return _reference(_reference_store, "refgpu", r)
 
 
 @pytest.fixture(scope="session")

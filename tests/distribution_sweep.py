@@ -1,7 +1,7 @@
 """Value-distribution sensitivity of the variable-base MSM (SURVEY §8d): the bucket load depends on the
 scalars. Device-resident ristretto MSM, n = 2^20, for uniform 252-bit scalars, all-ones scalars (every
 digit lands in ONE bucket per window), tiny scalars (one non-zero window), a boolean column and a column
-that is 99 % zeros. Run on a B200: python tests/distribution_sweep.py [log2 n]"""
+that is 99 % zeros. Run on a GPU: python tests/distribution_sweep.py [log2 n]"""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """Generates the committed golden fixtures from the REFERENCE's own CPU implementation
-(oracle/_ref, built from /root/reference by oracle/ref_build/Makefile). Run in the build container:
+(oracle/_ref, built from a reference checkout by oracle/ref_build/Makefile). Run where it is built:
 
     python tests/golden/make_golden.py
 

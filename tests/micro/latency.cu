@@ -1,6 +1,6 @@
 // Micro-benchmark (GPU box only): single-warp latency (cycles per operation in a dependent chain)
 // and full-chip throughput of the field / point primitives. Build:
-//   nvcc -std=c++17 -O3 -gencode arch=compute_100a,code=sm_100a --expt-relaxed-constexpr latency.cu -o latency
+//   nvcc -std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a --expt-relaxed-constexpr latency.cu -o latency
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../../blitzar_b200/csrc/curve.cuh"
@@ -77,8 +77,10 @@ __global__ void k_thr_addgen(Fe<8>* io, int iters) {
   for (int it = 0; it < iters; ++it) Ed25519::add_gen<SeqExec>(acc, acc, g, (it & 1) != 0);
   if (acc.X.l[0] == 0x12345678) io[8] = acc.Y;
 }
+static int g_sms = 0;
+static double g_hz = 0;  // the device's maximum SM clock
 template <class K> void thr_k(const char* name, K kern, Fe<8>* d, int threads, int blocks_per_sm) {
-  const int iters = 1000, blocks = 148 * blocks_per_sm;
+  const int iters = 1000, blocks = g_sms * blocks_per_sm;
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   kern<<<blocks, threads>>>(d, iters);
   cudaEventRecord(e0);
@@ -87,7 +89,7 @@ template <class K> void thr_k(const char* name, K kern, Fe<8>* d, int threads, i
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   double ops = (double)blocks * threads * iters;
   printf("throughput %-30s %d thr x %d blk/SM: %.2f G op/s (%.1f SM-cycles per warp-op)\n", name, threads, blocks_per_sm,
-         ops / ms * 1e-6, 1.965e9 * 148 / (ops / 32 / (ms * 1e-3)));
+         ops / ms * 1e-6, g_hz * g_sms / (ops / 32 / (ms * 1e-3)));
 }
 template <int OP> void lat(const char* name, Fe<8>* d, long long* dc, int threads) {
   const int iters = 200;
@@ -97,7 +99,7 @@ template <int OP> void lat(const char* name, Fe<8>* d, long long* dc, int thread
   printf("latency  %-28s %4d thr: %8.1f cycles/op\n", name, threads, (double)c / iters);
 }
 template <int OP> void thr(const char* name, Fe<8>* d) {
-  const int iters = 2000, blocks = 148 * 8, threads = 256;
+  const int iters = 2000, blocks = g_sms * 8, threads = 256;
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   k_thr<OP><<<blocks, threads>>>(d, iters);
   cudaEventRecord(e0);
@@ -105,10 +107,14 @@ template <int OP> void thr(const char* name, Fe<8>* d) {
   cudaEventRecord(e1); cudaEventSynchronize(e1);
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   double muls = (double)blocks * threads * iters;
-  printf("throughput %-26s: %.2f G mul/s (%.1f SM-cycles per warp-mul at 1.9 GHz)\n", name, muls / ms * 1e-6,
-         1.9e9 * 148 / (muls / 32 / (ms * 1e-3)));
+  printf("throughput %-26s: %.2f G mul/s (%.1f SM-cycles per warp-mul)\n", name, muls / ms * 1e-6,
+         g_hz * g_sms / (muls / 32 / (ms * 1e-3)));
 }
 int main() {
+  int khz = 0;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  g_hz = khz * 1e3;
   Fe<8>* d; long long* dc;
   cudaMalloc(&d, 64 * sizeof(Fe<8>)); cudaMalloc(&dc, 8);
   Fe<8> h[16];

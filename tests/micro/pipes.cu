@@ -1,5 +1,9 @@
 // Micro-benchmark: issue rates of the pipes the field multiplier can use (per SM per clock).
+//   nvcc -std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a pipes.cu -o pipes
+// Rates are per SM per clock at the SM clock sampled by nvidia-smi during the run (argv[1], MHz;
+// default: the device's maximum clock).
 #include <cstdio>
+#include <cstdlib>
 #include <cuda_runtime.h>
 typedef unsigned long long u64;
 typedef unsigned int u32;
@@ -52,8 +56,10 @@ template <int OP> __global__ void k(u64* out, int iters) {
   }
   out[blockIdx.x * blockDim.x + threadIdx.x] = a0 + a1 + a2 + a3 + a4 + a5 + a6 + a7 + (u64)(d0 + d1 + d2 + d3 + d4 + d5 + d6 + d7);
 }
+static int g_sms = 0;
+static double g_hz = 0;
 template <int OP> void run(const char* name, u64* d, double ops_per_iter) {
-  const int iters = 4000, blocks = 148 * 8, threads = 256;
+  const int iters = 4000, blocks = g_sms * 8, threads = 256;
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   k<OP><<<blocks, threads>>>(d, iters);
   cudaEventRecord(e0);
@@ -61,10 +67,16 @@ template <int OP> void run(const char* name, u64* d, double ops_per_iter) {
   cudaEventRecord(e1); cudaEventSynchronize(e1);
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   double ops = (double)blocks * threads * iters * ops_per_iter;
-  printf("%-34s %8.1f Gop/s  = %5.1f lane-ops/clk/SM at 1.965 GHz\n", name, ops / ms * 1e-6, ops / (ms * 1e-3) / 148 / 1.965e9);
+  printf("%-34s %8.1f Gop/s  = %5.1f lane-ops/clk/SM at %.3f GHz\n", name, ops / ms * 1e-6,
+         ops / (ms * 1e-3) / g_sms / g_hz, g_hz * 1e-9);
 }
-int main() {
-  u64* d; cudaMalloc(&d, 148 * 8 * 256 * 8);
+int main(int argc, char** argv) {
+  int khz = 0;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  g_hz = argc > 1 ? std::atof(argv[1]) * 1e6 : khz * 1e3;
+  printf("%d SMs\n", g_sms);
+  u64* d; cudaMalloc(&d, (size_t)g_sms * 8 * 256 * 8);
   run<0>("IMAD.WIDE.U32 (64 += 32x32)", d, 8);
   run<1>("DFMA.RZ", d, 8);
   run<2>("IMAD (32-bit)", d, 8);

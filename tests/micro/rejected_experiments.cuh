@@ -1,11 +1,11 @@
 // MEASURED AND REJECTED (round 1, DESIGN.md "What was measured and rejected"): kept out of the product,
 // next to the micro-benchmark that produced the numbers (tests/micro/latency.cu).
 //   * FP64-pipe field multiplication (F25519D) and the FP64 point accumulator built on it: exact, but
-//     82.8 vs 82.9 SM-cycles per warp-multiplication and 852 vs 808 per point addition;
-//   * one-level subtractive Karatsuba: 96.8 vs 83.0 SM-cycles per warp-multiplication.
+//     no faster per warp-multiplication and slower per point addition;
+//   * one-level subtractive Karatsuba: slower per warp-multiplication.
 // GF(2^255-19) multiplication on the FP64 pipe, for the bucket-accumulation kernel only.
 //
-// Measured on B200 (tests/micro/pipes.cu): IMAD.WIDE.U32 issues at 23 lane-ops/clk/SM, DFMA at 61.
+// tests/micro/pipes.cu measures the issue rates of IMAD.WIDE.U32 and DFMA this trade rests on.
 // A 52x52-bit product costs three FP64 instructions here (two DFMA.RZ + one DADD) against about
 // six-and-a-half IMAD.WIDE for the same bits, so the field multiplication of the hot loop moves to
 // double precision with EXACT integer semantics:

@@ -1,7 +1,7 @@
 """Throughput sweep n = 2^16 .. 2^24 (BASELINE.md §4): device-resident time and end-to-end C-ABI time
 per curve / API on one GPU, on the reference benchmarks' own generators (distinct points produced in
-HBM by b200_synthetic_generators_device — no tiling). Writes gpurun_out/sweep.json and prints a
-markdown table.   python tests/sweep.py   (SWEEP_MAX=22 to stop earlier)"""
+HBM by b200_synthetic_generators_device — no tiling). Prints a markdown table and, given a path,
+writes the rows there as JSON.   python tests/sweep.py [out.json]   (SWEEP_MAX=22 to stop earlier)"""
 import json
 import os
 import sys
@@ -81,8 +81,8 @@ for logn in range(16, max_log + 1, 2):
     do.free()
     print("done 2^%d" % logn, flush=True)
 
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(rows, open("gpurun_out/sweep.json", "w"), indent=1)
+if len(sys.argv) > 1:
+    json.dump(rows, open(sys.argv[1], "w"), indent=1)
 print("| path | n | device ms | terms/s (device) | GB/s algorithmic | e2e ms (pageable host) | terms/s (e2e) |")
 print("|---|---|---|---|---|---|---|")
 for r in rows:

@@ -92,7 +92,7 @@ def test_c3_full_size_closed_form(bb, refcpu):
 
 
 @pytest.mark.parametrize("curve", [2, 3])
-def test_c5_fixed_base_distinct_generators(bb, refcpu, curve):
+def test_c5_fixed_base_distinct_generators(bb, refcpu, port, curve):
     n = 1 << 18
     p2 = bb.synthetic_generators(curve, n, 0, projective=True)
     af = bb.synthetic_generators(curve, n, 0, projective=False)
@@ -100,7 +100,8 @@ def test_c5_fixed_base_distinct_generators(bb, refcpu, curve):
     s = _scalars(n, 5 + curve, 0x3F)
     res = h.fixed_multiexponentiation(32, 1, n, s)
     want = refcpu.commit(curve, [(s, 0)], af)
-    assert common.same(curve, refcpu.normalize(curve, res), want)
+    # the projective coordinates depend on the order of additions: normalised by the pinned C port
+    assert common.same(curve, port.normalize(curve, res), want)
     # two outputs of different widths in one packed call
     bt = [64, 17]
     row = (sum(bt) + 7) // 8
@@ -112,11 +113,11 @@ def test_c5_fixed_base_distinct_generators(bb, refcpu, curve):
         b = np.zeros((n, 8 * ((w + 7) // 8)), dtype=np.uint8)
         b[:, :w] = bits[:, lo:lo + w]
         cols.append((np.packbits(b, axis=1, bitorder="little"), 0))
-    assert common.same(curve, refcpu.normalize(curve, res), refcpu.commit(curve, cols, af))
+    assert common.same(curve, port.normalize(curve, res), refcpu.commit(curve, cols, af))
     h.free()
 
 
-def test_c5_full_size_closed_form(bb, refcpu):
+def test_c5_full_size_closed_form(bb, refcpu, port):
     n = 1 << 22
     buf = bb.DeviceBuffer(n * 96)
     bb.synthetic_generators_device(2, buf.ptr, n, 0, True)
@@ -127,4 +128,4 @@ def test_c5_full_size_closed_form(bb, refcpu):
     s = _scalars(n, 11, 0x3F)
     res = h.fixed_multiexponentiation(32, 1, n, s)
     h.free()
-    assert common.same(2, refcpu.normalize(2, res), common.closed_form_commitment(refcpu, 2, s))
+    assert common.same(2, port.normalize(2, res), common.closed_form_commitment(refcpu, 2, s))

@@ -307,14 +307,14 @@ print("multi-device ok")
 
 def test_columns_split_over_devices(bb):
     """BLITZAR_B200_DEVICES=k: independent columns run on k devices of this process (the reference
-    splits by output the same way, sxt/multiexp/pippenger2/multiexponentiation.h:248-287)."""
+    splits by output the same way, sxt/multiexp/pippenger2/multiexponentiation.h:248-287). With one
+    GPU, the test hook BLITZAR_B200_SHARED_DEVICES puts two shards on it."""
     import subprocess
     import sys
     import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, BLITZAR_B200_DEVICES=str(min(4, torch.cuda.device_count())),
+    env = dict(os.environ, BLITZAR_B200_DEVICES=str(max(2, min(4, torch.cuda.device_count()))),
+               BLITZAR_B200_SHARED_DEVICES="1" if torch.cuda.device_count() < 2 else "0",
                BLITZAR_B200_MIN_SHARD_TERMS="200")
     r = subprocess.run([sys.executable, "-c", _MULTI_DEVICE_SCRIPT, root], env=env, cwd=root,
                        capture_output=True, text=True, timeout=600)
