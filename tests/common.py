@@ -157,14 +157,150 @@ def dot_mod(scalars_u8, k_u64, r):
     return total % r
 
 
-def closed_form_commitment(refcpu, curve, scalars_u8, first=0):
+def closed_form_commitment(refcpu, curve, scalars_u8, first=0, k=None):
     """Reference commitment bytes of sum_i scalar_i * G_{first+i} through ONE reference scalar
-    multiplication of the subgroup generator."""
+    multiplication of the subgroup generator. k: discrete logs of generators that were edited after
+    synthesis (uint64 [n, 4], see GeneratorEdits); default the synthetic ones."""
     _, r, _, _, _ = curve_params(curve)
-    k = synth_scalars_k(scalars_u8.shape[0], first)
+    if k is None:
+        k = synth_scalars_k(scalars_u8.shape[0], first)
     e = dot_mod(scalars_u8, k, r)
     sc = np.frombuffer(e.to_bytes(32, "little"), dtype=np.uint8).reshape(1, 32)
     return refcpu.commit(curve, [(sc, 0)], subgroup_generator_affine(curve))
+
+
+# ---- degenerate Weierstrass generators (duplicates, negations, identities) --------------------------
+# byte offset of the infinity flag of an affine commitment generator {X, Y, infinity}
+AFFINE_FLAG = {1: 96, 2: 64, 3: 64}
+
+
+def _field_bytes(curve):
+    p, _, nl, _, _ = curve_params(curve)
+    return p, 8 * nl
+
+
+def negate_affine(curve, gens, rows):
+    """In place: y -> p - y (Montgomery form) on the given rows of an affine generator array of any
+    of the three Weierstrass layouts. Rows that are the identity are left alone."""
+    p, nb = _field_bytes(curve)
+    for i in np.arange(gens.shape[0])[rows]:
+        if gens[i, AFFINE_FLAG[curve]]:
+            continue
+        y = int.from_bytes(gens[i, nb:2 * nb].tobytes(), "little")
+        gens[i, nb:2 * nb] = np.frombuffer(((p - y) % p).to_bytes(nb, "little"), dtype=np.uint8)
+    return gens
+
+
+def set_identity(curve, gens, rows):
+    """In place: the group identity on the given rows. Affine arrays (stride 104 / 72) get the
+    infinity flag over zero coordinates (element_affine::identity()); projective arrays (stride 144 /
+    96) get {0, R, 0}, i.e. Z = 0 (element_p2::identity())."""
+    p, nb = _field_bytes(curve)
+    gens[rows] = 0
+    if gens.shape[1] == 3 * nb:
+        gens[rows, nb:2 * nb] = np.frombuffer(((1 << (8 * nb)) % p).to_bytes(nb, "little"),
+                                              dtype=np.uint8)
+    else:
+        gens[rows, AFFINE_FLAG[curve]] = 1
+    return gens
+
+
+def degenerate_buckets(port, curve):
+    """Affine generators and 1-byte columns whose terms all land in ONE bucket per column (scalar 1:
+    window 0, digit 1) holding nothing but copies of +-P, identities or, on bls12-381, the points
+    (0, +-2) of order 3 (x = 0 without being the identity). The bucket contents do not depend on the
+    order the entries are scattered in, only which pairs meet does.
+    Returns (gens, cols, equal): equal lists (column index, m) for buckets of m copies of P."""
+    p, nb = _field_bytes(curve)
+    n = 176
+    base = generators_for(port, curve, 2, seed=11)[0]
+    gens = np.repeat(base[:1], n, axis=0)              # rows 0..63: P
+    negate_affine(curve, gens, slice(65, 128, 2))      # rows 64..127: P, -P, P, -P, ...
+    set_identity(curve, gens, slice(129, 160, 2))      # rows 128..159: P, O, P, O, ...
+    gens[160:] = base[1]                               # rows 160..175: another point Q
+    if curve == 1:                                     # rows 160..167: (0, 2) (0, 2) (0, -2) ...
+        for i, sign in zip(range(160, 168), (1, 1, -1, 1, -1, -1, 1, 1)):
+            gens[i, :nb] = 0
+            gens[i, nb:2 * nb] = np.frombuffer((sign * 2 * (1 << (8 * nb)) % p).to_bytes(nb, "little"),
+                                               dtype=np.uint8)
+
+    def ones(rows):
+        col = np.zeros((n, 1), dtype=np.uint8)
+        col[rows] = 1
+        return (col, 0)
+
+    cols, equal = [], []
+    for m in (2, 4, 8, 16, 32, 64, 3, 5, 7):  # doublings at every level; real entries next to pads
+        equal.append((len(cols), m))
+        cols.append(ones(slice(0, m)))
+    cols += [ones(slice(64, 128)),   # cancellations at level 0, identity operands above
+             ones(slice(64, 69)),    # P - P + P - P + P
+             ones(slice(128, 160)),  # P next to identity generators
+             ones(slice(127, 162)),  # -P, then P / O, then Q (x = 0 on bls12-381)
+             ones(slice(160, 168)), ones(slice(160, 162)), ones(slice(161, 163))]
+    rng = np.random.default_rng(curve)
+    mix = rng.choice(np.array([1, 1, 1, 2, 0xFF], dtype=np.uint8), (n, 1))  # digits +-1 and 2, signed
+    cols.append((mix, 1))
+    return gens, cols, equal
+
+
+RISTRETTO_R = (1 << 252) + 27742317777372353535851937790883648493
+
+
+def cross_window_handle(port, curve, c, m=40):
+    """Projective handle generators and fixed-MSM scalars (2 outputs x 32 bytes) for a fixed-base
+    table of window c, whose windows share one bucket set: G_1 = 2^c G_0, G_2 = -2^c G_0 and
+    G_4 = -2^c G_3, G_5 = 2^c G_3, with scalars d 2^c, d, d (and e 2^c, e, e), so that window 1 of
+    G_0 (G_3) and window 0 of the other two land in the same bucket: a doubling and a cancellation
+    inside table mode. Output 1 is random over all m rows."""
+    r = RISTRETTO_R if curve == 0 else curve_params(curve)[1]
+    _, gens_p = generators_for(port, curve, m, seed=21)
+    gens_p = gens_p.copy()
+
+    def s32(v):
+        return np.frombuffer(v.to_bytes(32, "little"), dtype=np.uint8)
+
+    two_c = 1 << c
+    mult = np.concatenate([s32(two_c), s32(r - two_c)])[None]
+    for i, plus, minus in ((0, 1, 2), (3, 5, 4)):
+        gens_p[[plus, minus]] = port.fixed_msm(curve, gens_p[i:i + 1], 2, 1, mult, element_num_bytes=32)
+    rng = np.random.default_rng(c + 10 * curve)
+    sc = rng.integers(0, 256, (m, 2, 32), dtype=np.uint8)
+    sc[:, 0] = 0
+    for rows, digit in (((0, 1, 2), 5), ((3, 4, 5), 9)):
+        sc[rows[0], 0] = s32(digit << c)
+        sc[rows[1], 0] = sc[rows[2], 0] = s32(digit)
+    return gens_p, sc.reshape(m, 64)
+
+
+class GeneratorEdits:
+    """Row edits of synthetic affine generators G_i = k_i G (synthetic_generators) that keep the
+    discrete logs k'_i in step, so that closed_form_commitment(..., k=edits.k) stays exact."""
+
+    def __init__(self, curve, gens, first=0):
+        self.curve, self.gens = curve, gens
+        self.r = curve_params(curve)[1]
+        self.k = synth_scalars_k(gens.shape[0], first)
+
+    def _set_logs(self, rows, fn):
+        for i in np.arange(self.k.shape[0])[rows]:
+            v = fn(int.from_bytes(self.k[i].tobytes(), "little"))
+            self.k[i] = np.frombuffer(v.to_bytes(32, "little"), dtype=np.uint64)
+
+    def duplicate(self, dst, src):
+        """G_dst = G_src (k'_dst = k_src)."""
+        self.gens[dst] = self.gens[src]
+        self.k[dst] = self.k[src]
+
+    def negate(self, rows):
+        """G_i = -G_i (k'_i = r - k_i)."""
+        negate_affine(self.curve, self.gens, rows)
+        self._set_logs(rows, lambda v: (self.r - v) % self.r)
+
+    def identity(self, rows):
+        """G_i = O (k'_i = 0)."""
+        set_identity(self.curve, self.gens, rows)
+        self.k[rows] = 0
 
 
 def mt19937_bytes(seed, n, nbytes=32, top_mask=0x0F):

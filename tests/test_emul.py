@@ -139,6 +139,34 @@ def test_identity_generators_weierstrass(emul, port):
         assert common.same(curve, emul.commit(curve, cols, gens), port.commit(curve, cols, gens))
 
 
+@pytest.mark.parametrize("levels", [-1, 1, 3, 6])
+def test_identity_generators_in_pair_levels(emul, port, levels):
+    """Identity generators as operands of the batch-affine pair levels (a column of ones pairs them
+    with real points), and projective handle generators with Z = 0, with and without the table."""
+    rng = np.random.default_rng(4)
+    try:
+        emul.set_pairs(levels, 0)
+        for curve in (1, 2, 3):
+            gens, gens_p = common.generators_for(port, curve, 20)
+            gens, gens_p = gens.copy(), gens_p.copy()
+            common.set_identity(curve, gens, [0, 7, 19])
+            cols = common.random_columns(rng, 20, [(0, 32, 0), (0, 2, 0)])
+            cols.append((np.ones((20, 1), dtype=np.uint8), 0))
+            assert common.same(curve, emul.commit(curve, cols, gens), port.commit(curve, cols, gens))
+            common.set_identity(curve, gens_p, [0, 7, 19])
+            sc = rng.integers(0, 256, (20, 2 * 32), dtype=np.uint8)
+            sc[:, 32:] = 0
+            sc[:, 32] = 1
+            want = port.normalize(curve, port.fixed_msm(curve, gens_p, 2, 20, sc, element_num_bytes=32))
+            for table in (0, 10):
+                emul.set_table(table, 1 if table else 0)
+                got = emul.fixed_msm(curve, gens_p, 2, 20, sc, element_num_bytes=32)
+                assert common.same(curve, port.normalize(curve, got), want), (curve, table)
+    finally:
+        emul.set_pairs(-1, 0)
+        emul.set_table(0, 0)
+
+
 @pytest.mark.parametrize("curve", [0, 2])
 @pytest.mark.parametrize("num_ranges", [2, 3, 7])
 def test_generator_ranges_share_one_bucket_array(emul, port, curve, num_ranges):
@@ -287,7 +315,7 @@ def test_batch_affine_pair_levels(emul, port, curve):
     cols += [(ones, 0), (sg, 1)]
     want = port.commit(curve, cols, gens)
     try:
-        for c, levels, batch in ((4, 1, 4), (4, 3, 5), (6, 2, 32), (3, 5, 0), (2, 6, 64)):
+        for c, levels, batch in ((4, 1, 4), (4, 3, 5), (6, 2, 32), (3, 5, 0), (2, 6, 64), (0, 6, 1)):
             emul.set_tuning(window_bits=c)
             emul.set_pairs(levels, batch)
             assert common.same(curve, emul.commit(curve, cols, gens), want), (c, levels, batch)
@@ -298,4 +326,70 @@ def test_batch_affine_pair_levels(emul, port, curve):
     finally:
         emul.set_ranges(1)
         emul.set_tuning()
+        emul.set_pairs(-1, 0)
+
+
+@pytest.mark.parametrize("curve", [1, 2, 3])
+def test_degenerate_pair_level_buckets(emul, port, curve):
+    """Buckets of nothing but copies of +-P, identities and (bls12-381) the x = 0 points (0, +-2)
+    through every number of pair levels: doublings, cancellations and identity operands at every
+    level, in the fused next-level classification and in the rare-path gather of pass 1."""
+    gens, cols, equal = common.degenerate_buckets(port, curve)
+    want = port.commit(curve, cols, gens)
+    for j, m in equal:
+        assert common.same(curve, want[j:j + 1],
+                           port.commit(curve, [(np.array([[m]], dtype=np.uint8), 0)], gens[:1])), m
+    try:
+        for levels in (-1, 1, 2, 3, 4, 5, 6):
+            emul.set_pairs(levels, 0)
+            assert common.same(curve, emul.commit(curve, cols, gens), want), levels
+    finally:
+        emul.set_pairs(-1, 0)
+
+
+@pytest.mark.parametrize("curve", [0, 1, 2, 3])
+@pytest.mark.parametrize("window_bits", [10, 16])
+def test_fixed_base_table_cross_window_collisions(emul, port, curve, window_bits):
+    """Table mode shares one bucket set over all windows, so with G_j = +-2^c G_i window 1 of i and
+    window 0 of j meet in one bucket with equal x: doublings and cancellations inside the pair levels
+    (ristretto255, with complete formulas and no pair levels, is the control)."""
+    gens_p, sc = common.cross_window_handle(port, curve, window_bits)
+    m = gens_p.shape[0]
+    want = port.normalize(curve, port.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32))
+    try:
+        emul.set_table(window_bits, 1)
+        for levels in (-1, 1, 2, 3):
+            emul.set_pairs(levels, 0)
+            got = emul.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
+            assert common.same(curve, port.normalize(curve, got), want), levels
+    finally:
+        emul.set_table(0, 0)
+        emul.set_pairs(-1, 0)
+
+
+@pytest.mark.parametrize("curve", [1, 2, 3])
+def test_edited_synthetic_generators_keep_the_closed_form(emul, port, curve):
+    """Duplicated, negated and identity rows of synthetic generators, with their discrete logs kept
+    in step (the bookkeeping of the full-size device test), still give the closed form."""
+    n = 400
+    gens = emul.synth_generators(curve, n)
+    ed = common.GeneratorEdits(curve, gens)
+    rng = np.random.default_rng(curve)
+    s = rng.integers(0, 256, (n, 32), dtype=np.uint8)
+    rows = np.arange(16, n, 16)
+    ed.duplicate(rows, rows - 1)
+    s[rows] = s[rows - 1]
+    ed.duplicate(rows[:-1] + 1, rows[:-1])
+    ed.negate(rows[:-1] + 1)
+    s[rows[:-1] + 1] = s[rows[:-1]]
+    ed.duplicate(slice(200, 264), 200)
+    s[200:264] = 0
+    s[200:264, 0] = 1
+    ed.identity(slice(5, n, 31))
+    want = port.commit(curve, [(s, 0)], gens)
+    assert common.same(curve, common.closed_form_commitment(port, curve, s, k=ed.k), want)
+    try:
+        emul.set_pairs(2, 0)
+        assert common.same(curve, emul.commit(curve, [(s, 0)], gens), want)
+    finally:
         emul.set_pairs(-1, 0)
