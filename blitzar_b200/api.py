@@ -38,7 +38,7 @@ B200_SYMBOLS = [
     "b200_profile_read", "b200_set_reduce_groups", "b200_stream",
     "b200_synthetic_generators_device", "b200_commit_host_partials",
     "b200_fixed_msm_host_partials", "b200_multiexp_handle_new_device",
-    "b200_selftest_lane_arithmetic",
+    "b200_selftest_lane_arithmetic", "b200_selftest_sort",
 ]
 
 
@@ -267,6 +267,20 @@ def commit_device(curve_id, columns_shape, scalar_ptrs, generators_ptr, out_comm
 def selftest_lane_arithmetic(warps=64, seed=1):
     lib().b200_selftest_lane_arithmetic.restype = C.c_uint
     return int(lib().b200_selftest_lane_arithmetic(C.c_uint(warps), C.c_uint(seed)))
+
+
+def selftest_sort(columns_shape, scalar_ptrs, window_bits=0):
+    """b200_selftest_sort over device columns (list of (n, element_nbytes, is_signed) + pointers):
+    the number of buckets on which the atomic and the binned sort disagree."""
+    num = len(columns_shape)
+    arr = (sxt_sequence_descriptor * max(1, num))()
+    for i, (n, nbytes, is_signed) in enumerate(columns_shape):
+        arr[i].element_nbytes = nbytes
+        arr[i].n = n
+        arr[i].data = scalar_ptrs[i]
+        arr[i].is_signed = int(is_signed)
+    lib().b200_selftest_sort.restype = C.c_uint
+    return int(lib().b200_selftest_sort(arr, C.c_uint(num), C.c_uint(window_bits)))
 
 
 def synthetic_generators_device(curve_id, out_ptr, n, first=0, projective=False):

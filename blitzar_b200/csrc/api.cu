@@ -66,6 +66,8 @@ EngineCtx ctx_of(const State& st) {
     c.opt.lane_tail = (u32)std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_SCATTER_WM"))
     c.opt.scatter_window_major = (u32)std::atoi(env);
+  if (const char* env = std::getenv("BLITZAR_B200_SORT"))  // 0 atomic, 1 binned (large), 2 binned
+    c.opt.sort_path = (u32)std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_PAIR_LEVELS"))  // batch-affine levels (-1 = auto)
     c.opt.pair_levels = std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_PAIR_BATCH"))
@@ -1246,6 +1248,14 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);
+}
+unsigned b200_selftest_sort(const sxt_sequence_descriptor* columns, unsigned num,
+                            unsigned window_bits) {
+  std::lock_guard<std::mutex> lock(g_mutex);
+  require_init("b200_selftest_sort");
+  B200_REQUIRE(num == 0 || columns != nullptr, "columns == nullptr");
+  B200_REQUIRE(window_bits <= 20, "window_bits in 0..20");
+  return selftest_sort(ctx(), columns, num, window_bits);
 }
 void b200_set_reduce_groups(unsigned g1, unsigned gn) {
   std::lock_guard<std::mutex> lock(g_mutex);

@@ -23,6 +23,19 @@ unsigned selftest_lane_arithmetic(const EngineCtx& ctx, unsigned warps, unsigned
   return 0;
 #endif
 }
+unsigned selftest_sort(const EngineCtx& ctx, const sxt_sequence_descriptor* d, unsigned num,
+                       unsigned window_bits) {
+  std::vector<ColumnDesc> cols(num);
+  for (unsigned i = 0; i < num; ++i) {
+    cols[i] = ColumnDesc{};
+    cols[i].base = d[i].data;
+    cols[i].row_stride = d[i].element_nbytes;
+    cols[i].bit_width = 8u * d[i].element_nbytes;
+    cols[i].n = (u32)d[i].n;
+    cols[i].is_signed = d[i].is_signed ? 1u : 0u;
+  }
+  return sort_selftest(ctx.s, std::move(cols), window_bits);
+}
 void ipa_prove(const EngineCtx& ctx, uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value,
                uint8_t* transcript203, uint64_t n, uint64_t generators_offset,
                const uint8_t* a_vector, const uint8_t* b_vector) {

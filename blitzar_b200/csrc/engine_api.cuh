@@ -27,6 +27,9 @@ struct MsmOptions {
   u32 gens_normalized = 0;  // set per call: the generator array is a fixed-base table (Z = 1 entries)
   u32 lane_tail = 1;  // warp-cooperative (lane-sliced) Horner / encoding kernels for ed25519
   u32 scatter_window_major = 0;  // scatter with one thread per (window, term), window-major
+  // bucket sort of the entries: 0 = atomic count + scan + scatter; 1 = binned sort (msm.cuh) for
+  // unpadded passes of at least kBinnedSortMinEntries entries; 2 = binned whenever it applies
+  u32 sort_path = 1;
   u32 table_policy = 0;  // fixed-base tables: 0 = cost model decides, 1 = whenever available, 2 = never
 };
 
@@ -143,6 +146,9 @@ int ipa_verify(const EngineCtx& ctx, uint8_t* transcript203, uint64_t n,
 // lane-sliced field arithmetic self-test (lanefield.cuh): number of mismatching checks over
 // `warps` warps of pseudo-random / edge-case operands
 unsigned selftest_lane_arithmetic(const EngineCtx& ctx, unsigned warps, unsigned seed);
+// atomic against binned bucket sort of the same device columns (msm.cuh sort_selftest)
+unsigned selftest_sort(const EngineCtx& ctx, const sxt_sequence_descriptor* d, unsigned num,
+                       unsigned window_bits);
 
 // built-in ristretto generators g(first .. first+n) into the device generator layout
 void launch_builtin_generators(const EngineCtx& ctx, void* gens, uint64_t first, uint64_t n);

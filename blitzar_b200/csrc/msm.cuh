@@ -300,6 +300,322 @@ inline void exclusive_scan(u32* data, u64 n, stream_t s, u32 chunk = kScanChunkF
   dev_free(partial, s);
 }
 
+#if defined(__CUDACC__) && !defined(B200_EMULATE)
+#define B200_BINNED_SORT 1
+// ---- binned sort of the (term, window) entries (block-cooperative, CUDA only) ----------------------
+// The same output as CountBody -> exclusive_scan -> ScatterBody (entries sorted by key, counts[k] = END
+// offset of bucket k, d_m[0] = M) without a global atomic or a scattered 8-byte store per entry:
+//   1. MicroCountBody: per tile of terms, a shared-memory histogram of micro-bins (key >> shift),
+//      flushed with one global atomic per non-zero counter
+//   2. PlanBinsBody: one block scans the micro-bins and groups consecutive ones into bins of at most
+//      kBinCap entries and kBinSpan keys; a micro-bin above kBinCap / 2 entries is a bin of its own
+//   3. CoarseScatterBody: per tile, ranks its entries by bin in shared memory, reserves the tile's run
+//      in every bin with one global atomic, and writes the runs to a temporary array
+//   4. BinSortBody: per bin, counting sort by key in shared memory, final positions bin start + local
+//      offset, and the bins' bucket end offsets. A bin above kBinCap entries (one micro-bin holding a
+//      very dense bucket) is sorted the same way out of global memory.
+constexpr u32 kMicroBins = 16384, kBinCap = 8192, kBinSpan = 4096, kMaxBinShift = 12;
+// below this many entries the atomic path's fewer launches win (MsmOptions::sort_path = 1)
+constexpr u64 kBinnedSortMinEntries = 1ull << 20;
+
+// exclusive prefix of v over the block (kBlock threads, all of them call it); *total = block sum
+template <int kBlock> __device__ u32 block_exclusive_scan(u32 v, u32* warp_sums, u32* total) {
+  const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  u32 x = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const u32 y = __shfl_up_sync(0xffffffffu, x, d);
+    if (lane >= (u32)d)
+      x += y;
+  }
+  if (lane == 31)
+    warp_sums[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    u32 w = lane < kBlock / 32 ? warp_sums[lane] : 0u;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const u32 y = __shfl_up_sync(0xffffffffu, w, d);
+      if (lane >= (u32)d)
+        w += y;
+    }
+    if (lane < kBlock / 32)
+      warp_sums[lane] = w;
+  }
+  __syncthreads();
+  const u32 pre = (warp ? warp_sums[warp - 1] : 0u) + x - v;
+  *total = warp_sums[kBlock / 32 - 1];
+  __syncthreads();  // warp_sums may be reused right away
+  return pre;
+}
+
+// f(key, entry) for every non-zero digit of term tid (entry as ScatterBody writes it)
+template <class Fn>
+__device__ void for_each_entry(const ColumnDesc* cols, const u64* col_start, u32 ncols, u32 c,
+                               u32 nbuckets, u64 tid, Fn f) {
+  const u32 j = column_of(col_start, ncols, tid);
+  const ColumnDesc col = cols[j];
+  const u64 i = tid - col_start[j];
+  u32 v[8];
+  bool neg;
+  load_scalar_bits(v, neg, col, i);
+  const u32 ii = (u32)i, tn = col.table_n;
+  for_each_digit(v, neg, col, c, nbuckets, [&](u32 key, bool negate, u32 w) {
+    f(key, ((u64)key << 32) | (u64)(((ii + w * tn) << 1) | (negate ? 1u : 0u)));
+  });
+}
+
+struct MicroCountBody {
+  static constexpr int kBlock = 512;
+  const ColumnDesc* cols;
+  const u64* col_start;
+  u32 ncols, c, nbuckets;
+  u64 total_terms;
+  u32 tile, shift, nmicro;
+  u32* micro_counts;  // [nmicro], zeroed
+  __device__ void run(u32 b, unsigned char* smem) const {
+    u32* h = (u32*)smem;
+    for (u32 m = threadIdx.x; m < nmicro; m += kBlock)
+      h[m] = 0;
+    __syncthreads();
+    const u64 lo = (u64)b * tile, hi = lo + tile < total_terms ? lo + tile : total_terms;
+    const u32 sh = shift;
+    for (u64 t = lo + threadIdx.x; t < hi; t += kBlock)
+      for_each_entry(cols, col_start, ncols, c, nbuckets, t,
+                     [h, sh](u32 key, u64) { atomicAdd(&h[key >> sh], 1u); });
+    __syncthreads();
+    for (u32 m = threadIdx.x; m < nmicro; m += kBlock)
+      if (h[m])
+        atomicAdd(&micro_counts[m], h[m]);
+  }
+};
+
+struct PlanBinsBody {
+  static constexpr int kBlock = 1024;
+  const u32* micro_counts;
+  u32 nmicro, span_micro;  // a bin never crosses a multiple of span_micro micro-bins
+  u64 nkeys;
+  u32* bin_of;      // [nmicro]: bin of every micro-bin
+  u32* bin_start;   // [nmicro + 1]: first slot of bin b; [nbins] = M
+  u32* bin_micro;   // [nmicro + 1]: first micro-bin of bin b; [nbins] = nmicro
+  u32* bin_cursor;  // [nmicro]: = bin_start, consumed by the coarse scatter
+  u32* nbins_out;
+  u32* counts;  // counts[nkeys] = M
+  u32* d_m;     // d_m[0] = M
+  __device__ bool starts_bin(const u32* st, u32 m) const {
+    constexpr u32 H = kBinCap / 2;
+    return m == 0 || m % span_micro == 0 || micro_counts[m] > H || micro_counts[m - 1] > H ||
+           st[m] / H != st[m - 1] / H;
+  }
+  __device__ void run(u32, unsigned char* smem) const {
+    __shared__ u32 ws[32];
+    u32* st = (u32*)smem;  // exclusive prefix of every micro-bin
+    const u32 per = (nmicro + kBlock - 1) / kBlock, m0 = min(threadIdx.x * per, nmicro),
+              m1 = min(m0 + per, nmicro);
+    u32 sum = 0;
+    for (u32 m = m0; m < m1; ++m)
+      sum += micro_counts[m];
+    u32 total;
+    u32 run = block_exclusive_scan<kBlock>(sum, ws, &total);
+    for (u32 m = m0; m < m1; ++m) {
+      st[m] = run;
+      run += micro_counts[m];
+    }
+    __syncthreads();
+    u32 nf = 0;
+    for (u32 m = m0; m < m1; ++m)
+      nf += starts_bin(st, m) ? 1u : 0u;
+    u32 nbins;
+    u32 id = block_exclusive_scan<kBlock>(nf, ws, &nbins);
+    for (u32 m = m0; m < m1; ++m) {
+      if (starts_bin(st, m)) {
+        bin_start[id] = st[m];
+        bin_micro[id] = m;
+        bin_cursor[id] = st[m];
+        ++id;
+      }
+      bin_of[m] = id - 1;
+    }
+    if (threadIdx.x == 0) {
+      bin_start[nbins] = total;
+      bin_micro[nbins] = nmicro;
+      *nbins_out = nbins;
+      counts[nkeys] = total;
+      d_m[0] = total;
+    }
+  }
+};
+
+// A tile's entries are ordered by bin in shared memory and each bin's run is written in one burst,
+// so that a 32-byte sector of the temporary array is complete (or meets its neighbour run) while it
+// is still in L2; written entry by entry as the digits are recoded, the runs of all resident tiles
+// stay partially written for the whole kernel and the array (M x 8 B) does not fit in L2.
+struct CoarseScatterBody {
+  static constexpr int kBlock = 1024;
+  const ColumnDesc* cols;
+  const u64* col_start;
+  u32 ncols, c, nbuckets;
+  u64 total_terms;
+  u32 tile, shift, nmicro;  // tile * (windows of a term) <= the staging capacity
+  const u32* bin_of;
+  const u32* nbins_ptr;
+  u32* bin_cursor;
+  u64* tmp;
+  __device__ void run(u32 b, unsigned char* smem) const {
+    __shared__ u32 ws[32];
+    u32* h = (u32*)smem;       // per bin: the tile's count, then its next staging slot
+    u32* delta = h + nmicro;   // per bin: global slot - staging slot of the bin's run
+    u64* stage = (u64*)(delta + nmicro + (nmicro & 1u));
+    const u32 nbins = *nbins_ptr;
+    for (u32 k = threadIdx.x; k < nbins; k += kBlock)
+      h[k] = 0;
+    __syncthreads();
+    const u64 lo = (u64)b * tile, hi = lo + tile < total_terms ? lo + tile : total_terms;
+    const u32 sh = shift;
+    const u32* map = bin_of;
+    for (u64 t = lo + threadIdx.x; t < hi; t += kBlock)
+      for_each_entry(cols, col_start, ncols, c, nbuckets, t,
+                     [h, sh, map](u32 key, u64) { atomicAdd(&h[__ldg(&map[key >> sh])], 1u); });
+    __syncthreads();
+    const u32 per = (nbins + kBlock - 1) / kBlock, k0 = min(threadIdx.x * per, nbins),
+              k1 = min(k0 + per, nbins);
+    u32 sum = 0;
+    for (u32 k = k0; k < k1; ++k)
+      sum += h[k];
+    u32 size;
+    u32 run = block_exclusive_scan<kBlock>(sum, ws, &size);
+    for (u32 k = k0; k < k1; ++k) {
+      const u32 n = h[k];
+      if (n)
+        delta[k] = atomicAdd(&bin_cursor[k], n) - run;
+      h[k] = run;
+      run += n;
+    }
+    __syncthreads();
+    for (u64 t = lo + threadIdx.x; t < hi; t += kBlock)
+      for_each_entry(cols, col_start, ncols, c, nbuckets, t, [h, sh, map, stage](u32 key, u64 e) {
+        stage[atomicAdd(&h[__ldg(&map[key >> sh])], 1u)] = e;
+      });
+    __syncthreads();
+    for (u32 i = threadIdx.x; i < size; i += kBlock) {
+      const u64 e = stage[i];
+      tmp[delta[__ldg(&map[(u32)(e >> 32) >> sh])] + i] = e;  // u32 wrap-around: slot < 2^32
+    }
+  }
+};
+
+struct BinSortBody {
+  static constexpr int kBlock = 1024;
+  static constexpr size_t kSmem = 2 * kBinCap * sizeof(u64) + kBinSpan * sizeof(u32);
+  const u64* tmp;
+  const u32* bin_start;
+  const u32* bin_micro;
+  const u32* nbins_ptr;
+  u32 shift;
+  u64 nkeys;
+  u64* entries;
+  u32* counts;  // END offset of every bucket
+  __device__ void run(u32 b, unsigned char* smem) const {
+    __shared__ u32 ws[32];
+    if (b >= *nbins_ptr)
+      return;
+    u64* ent = (u64*)smem;
+    u32* h = (u32*)(smem + 2 * kBinCap * sizeof(u64));
+    const u32 lo = bin_start[b], size = bin_start[b + 1] - lo;
+    const u64 klo = (u64)bin_micro[b] << shift, khi_m = (u64)bin_micro[b + 1] << shift;
+    const u32 span = (u32)((khi_m < nkeys ? khi_m : nkeys) - klo);
+    const bool local = size <= kBinCap;  // else: a dense micro-bin, sorted out of global memory
+    for (u32 k = threadIdx.x; k < span; k += kBlock)
+      h[k] = 0;
+    if (local) {  // plain copy first: the loads stay independent of the histogram atomics
+#pragma unroll 4
+      for (u32 i = threadIdx.x; i < size; i += kBlock)
+        ent[i] = tmp[(u64)lo + i];
+    }
+    __syncthreads();
+    for (u32 i = threadIdx.x; i < size; i += kBlock) {
+      const u64 e = local ? ent[i] : tmp[(u64)lo + i];
+      atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u);
+    }
+    __syncthreads();
+    const u32 per = (span + kBlock - 1) / kBlock, k0 = min(threadIdx.x * per, span),
+              k1 = min(k0 + per, span);
+    u32 sum = 0;
+    for (u32 k = k0; k < k1; ++k)
+      sum += h[k];
+    u32 total;
+    u32 run = block_exclusive_scan<kBlock>(sum, ws, &total);
+    for (u32 k = k0; k < k1; ++k) {
+      const u32 n = h[k];
+      h[k] = run;
+      run += n;
+      counts[klo + k] = lo + run;
+    }
+    __syncthreads();
+    if (!local) {
+      for (u32 i = threadIdx.x; i < size; i += kBlock) {
+        const u64 e = tmp[(u64)lo + i];
+        entries[(u64)lo + atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u)] = e;
+      }
+      return;
+    }
+    // ordered in shared memory, then written out contiguously: one store per 32 entries of a warp
+    // instead of one 32-byte sector per entry
+    u64* sorted = ent + kBinCap;
+    for (u32 i = threadIdx.x; i < size; i += kBlock) {
+      const u64 e = ent[i];
+      sorted[atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u)] = e;
+    }
+    __syncthreads();
+    for (u32 i = threadIdx.x; i < size; i += kBlock)
+      entries[(u64)lo + i] = sorted[i];
+  }
+};
+
+// micro-bin shift for nkeys keys; > kMaxBinShift: too many keys for the binned sort
+inline u32 binned_sort_shift(u64 nkeys) {
+  u32 shift = 0;
+  while ((nkeys + (1ull << shift) - 1) >> shift > kMicroBins)
+    ++shift;
+  return shift;
+}
+
+// Binned sort of the entries of terms [0, total_terms) of d_cols into entries / counts / d_m[0].
+inline void binned_sort(stream_t s, const ColumnDesc* d_cols, const u64* d_col_start, u32 ncols,
+                        u32 c, u32 nbuckets, u64 total_terms, u64 max_entries, u32 max_windows,
+                        u64 nkeys, u64* entries, u32* counts, u32* d_m) {
+  const u32 shift = binned_sort_shift(nkeys);
+  const u32 nmicro = (u32)((nkeys + (1ull << shift) - 1) >> shift);
+  const u32 span_micro = std::max(1u, kBinSpan >> shift);
+  // workspace: micro_counts, bin_of, bin_cursor [nmicro]; bin_start, bin_micro [nmicro + 1]; nbins
+  u32* ws = (u32*)dev_alloc((5ull * nmicro + 3) * sizeof(u32), s);
+  u32 *micro_counts = ws, *bin_of = ws + nmicro, *bin_cursor = ws + 2ull * nmicro,
+      *bin_start = ws + 3ull * nmicro, *bin_micro = ws + 4ull * nmicro + 1,
+      *nbins = ws + 5ull * nmicro + 2;
+  u64* tmp = (u64*)dev_alloc(std::max<u64>(max_entries, 1) * sizeof(u64), s);
+  dev_zero(micro_counts, nmicro * sizeof(u32), s);
+  const u64 count_tile = 4096;
+  launch_blocks(MicroCountBody{d_cols, d_col_start, ncols, c, nbuckets, total_terms,
+                               (u32)count_tile, shift, nmicro, micro_counts},
+                (total_terms + count_tile - 1) / count_tile, nmicro * sizeof(u32), s);
+  launch_blocks(PlanBinsBody{micro_counts, nmicro, span_micro, nkeys, bin_of, bin_start, bin_micro,
+                             bin_cursor, nbins, counts, d_m},
+                1, nmicro * sizeof(u32), s);
+  // scatter tiles: as many terms as the shared memory left by the two per-bin arrays can stage
+  const size_t scatter_smem = 220 * 1024;
+  const size_t bin_bytes = (2ull * nmicro + 2) * sizeof(u32);
+  const u64 stage_entries = (scatter_smem - bin_bytes) / sizeof(u64);
+  const u64 scatter_tile = std::max<u64>(1, stage_entries / max_windows);
+  launch_blocks(CoarseScatterBody{d_cols, d_col_start, ncols, c, nbuckets, total_terms,
+                                  (u32)scatter_tile, shift, nmicro, bin_of, nbins, bin_cursor, tmp},
+                (total_terms + scatter_tile - 1) / scatter_tile, scatter_smem, s);
+  launch_blocks(BinSortBody{tmp, bin_start, bin_micro, nbins, shift, nkeys, entries, counts}, nmicro,
+                BinSortBody::kSmem, s);
+  dev_free(tmp, s);
+  dev_free(ws, s);
+}
+#endif
+
 template <class C> struct FillIdentityBody {
   static constexpr int kBlock = 256;
   typename C::Point* p;
@@ -853,6 +1169,67 @@ inline MsmPlan msm_make_plan(std::vector<ColumnDesc> cols, const MsmOptions& opt
   return p;
 }
 
+// Sorts the entries of `cols` (host descriptors over device scalars, window width c; 0 = automatic)
+// with the atomic path and with the binned path, and returns the number of buckets whose end offset
+// or entry multiset differs between the two (0 = agree; ~0u when the binned path does not apply).
+inline unsigned sort_selftest(stream_t s, std::vector<ColumnDesc> cols, u32 c) {
+#ifdef B200_BINNED_SORT
+  MsmOptions opt;
+  opt.window_bits = c;
+  const MsmPlan plan = msm_make_plan(std::move(cols), opt, 160);
+  if (plan.total_terms == 0 || binned_sort_shift(plan.nkeys) > kMaxBinShift)
+    return ~0u;
+  const u32 ncols = plan.ncols;
+  const u64 nkeys = plan.nkeys, M = plan.total_entries;
+  std::vector<u64> col_start(ncols + 1, 0);
+  for (u32 j = 0; j < ncols; ++j)
+    col_start[j + 1] = col_start[j] + plan.cols[j].n;
+  DevBuf<ColumnDesc> d_cols(ncols, s);
+  DevBuf<u64> d_col_start(ncols + 1, s);
+  copy_h2d(d_cols.p, plan.cols.data(), ncols * sizeof(ColumnDesc), s);
+  copy_h2d(d_col_start.p, col_start.data(), (ncols + 1) * sizeof(u64), s);
+  DevBuf<u32> counts_a(nkeys + 1, s), counts_b(nkeys + 1, s), d_m(16, s);
+  DevBuf<u64> entries_a(M + 1, s), entries_b(M + 1, s);
+  dev_zero(counts_a.p, (nkeys + 1) * sizeof(u32), s);
+  launch(CountBody{d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, counts_a.p},
+         plan.total_terms, s);
+  exclusive_scan(counts_a.p, nkeys + 1, s);
+  launch(ScatterBody{d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, counts_a.p, entries_a.p, 0},
+         plan.total_terms, s);
+  u32 max_windows = 0;
+  for (const auto& col : plan.cols)
+    max_windows = std::max(max_windows, col.n ? col.num_windows : 0u);
+  binned_sort(s, d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, plan.total_terms, M,
+              max_windows, nkeys, entries_b.p, counts_b.p, d_m.p);
+  std::vector<u32> ca(nkeys + 1), cb(nkeys + 1), m(1);
+  std::vector<u64> ea(M), eb(M);
+  copy_d2h(ca.data(), counts_a.p, (nkeys + 1) * sizeof(u32), s);
+  copy_d2h(cb.data(), counts_b.p, (nkeys + 1) * sizeof(u32), s);
+  copy_d2h(m.data(), d_m.p, sizeof(u32), s);
+  copy_d2h(ea.data(), entries_a.p, M * sizeof(u64), s);
+  copy_d2h(eb.data(), entries_b.p, M * sizeof(u64), s);
+  stream_sync(s);
+  unsigned bad = m[0] == ca[nkeys] ? 0u : 1u;  // M: counts[nkeys] of the atomic path
+  for (u64 k = 0; k < nkeys; ++k) {
+    const u32 lo = k ? ca[k - 1] : 0u, hi = ca[k];
+    if (cb[k] != hi || hi < lo || hi > M) {
+      ++bad;
+      continue;
+    }
+    std::sort(ea.begin() + lo, ea.begin() + hi);
+    std::sort(eb.begin() + lo, eb.begin() + hi);
+    if (!std::equal(ea.begin() + lo, ea.begin() + hi, eb.begin() + lo))
+      ++bad;
+  }
+  return bad;
+#else
+  (void)s;
+  (void)cols;
+  (void)c;
+  return ~0u;
+#endif
+}
+
 // Optional per-range hook: called before the terms [begin, end) are touched (the C-ABI layer uses
 // it to wait for that range's host-to-device copies and to ingest its generators).
 struct RangeHook {
@@ -905,9 +1282,6 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
   const u64* d_col_start = (const u64*)(d_stage + desc_bytes);
 
   StageRange nvtx_sort("msm: digit count + scan + scatter");
-  u32* d_counts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
-  dev_zero(d_counts, (nkeys + 1) * sizeof(u32), s);
-  launch(CountBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts}, total_terms, s);
   // Batch-affine pair levels (short Weierstrass curves, large passes): L levels, buckets padded to
   // multiples of 2^L slots; L from the mean bucket load so that pads stay below ~1/4 of the slots.
   u32 L = 0;
@@ -923,28 +1297,45 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
   }
   const u64 slots_max =
       L ? ((max_entries + nkeys * ((1ull << L) - 1) + (1ull << L) - 1) >> L) << L : max_entries;
+  u32* d_counts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
+  u32* d_m = (u32*)dev_alloc(16 * sizeof(u32), s);
+  u64* d_entries = (u64*)dev_alloc(slots_max * sizeof(u64), s);
   u32* d_starts = nullptr;
+  u32 max_windows = 0;
+  for (u32 j = 0; j < ncols; ++j)
+    max_windows = std::max(max_windows, cols[j].n ? cols[j].num_windows : 0u);
+  bool binned = false;
+#ifdef B200_BINNED_SORT
+  binned = L == 0 && opt.sort_path != 0 && binned_sort_shift(nkeys) <= kMaxBinShift &&
+           (opt.sort_path == 2 || max_entries >= kBinnedSortMinEntries);
+#endif
+  if (binned) {
+#ifdef B200_BINNED_SORT
+    binned_sort(s, d_cols, d_col_start, ncols, c, nbuckets, total_terms, max_entries, max_windows,
+                nkeys, d_entries, d_counts, d_m);
+#endif
+  } else {
+    dev_zero(d_counts, (nkeys + 1) * sizeof(u32), s);
+    launch(CountBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts}, total_terms, s);
+  }
   if (L) {
     launch(WindowUsedFromCountsBody{d_counts, nkeys, nbuckets, d_window_used}, (nkeys + 255) / 256, s);
     launch(PadCountsBody{d_counts, (1u << L) - 1u}, nkeys, s);
   }
-  exclusive_scan(d_counts, nkeys + 1, s);  // d_counts[nkeys] = number of (padded) entries
-  u32* d_m = (u32*)dev_alloc(16 * sizeof(u32), s);
-  copy_d2d(d_m, d_counts + nkeys, sizeof(u32), s);
-  if (L) {
-    d_starts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
-    copy_d2d(d_starts, d_counts, (nkeys + 1) * sizeof(u32), s);
+  if (!binned) {
+    exclusive_scan(d_counts, nkeys + 1, s);  // d_counts[nkeys] = number of (padded) entries
+    copy_d2d(d_m, d_counts + nkeys, sizeof(u32), s);
+    if (L) {
+      d_starts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
+      copy_d2d(d_starts, d_counts, (nkeys + 1) * sizeof(u32), s);
+    }
+    if (opt.scatter_window_major && max_windows > 1)
+      launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, total_terms},
+             total_terms * max_windows, s);
+    else
+      launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, 0},
+             total_terms, s);
   }
-  u64* d_entries = (u64*)dev_alloc(slots_max * sizeof(u64), s);
-  u32 max_windows = 0;
-  for (u32 j = 0; j < ncols; ++j)
-    max_windows = std::max(max_windows, cols[j].n ? cols[j].num_windows : 0u);
-  if (opt.scatter_window_major && max_windows > 1)
-    launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, total_terms},
-           total_terms * max_windows, s);
-  else
-    launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, 0},
-           total_terms, s);
   // d_counts[k] is now the END offset of bucket k's real entries
   if (L)
     launch(FillPadsBody{d_starts, d_counts, d_entries}, nkeys, s);

@@ -120,6 +120,28 @@ template <class Body> inline void launch(const Body& body, u64 n, stream_t s) {
   B200_CUDA(cudaGetLastError());
   ++LaunchCounter::value();
 }
+// Block-cooperative kernels: every thread of block b runs body.run(b, smem), with `smem_bytes` of
+// dynamic shared memory. Above the 48 KB default the kernel's limit is raised first (per device: the
+// attribute belongs to the calling thread's current device).
+template <class Body> __global__ void __launch_bounds__(Body::kBlock) k_block(Body body) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  body.run(blockIdx.x, smem);
+}
+template <class Body>
+inline void launch_blocks(const Body& body, u64 blocks, size_t smem_bytes, stream_t s) {
+  if (blocks == 0)
+    return;
+  B200_REQUIRE(blocks < (1ull << 31), "grid too large");
+  static thread_local size_t raised = 48 * 1024;
+  if (smem_bytes > raised) {
+    B200_CUDA(cudaFuncSetAttribute(k_block<Body>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)smem_bytes));
+    raised = smem_bytes;
+  }
+  k_block<Body><<<(unsigned)blocks, Body::kBlock, smem_bytes, s>>>(body);
+  B200_CUDA(cudaGetLastError());
+  ++LaunchCounter::value();
+}
 inline void* dev_alloc(size_t bytes, stream_t s) {
   void* p = nullptr;
   B200_CUDA(cudaMallocAsync(&p, bytes ? bytes : 16, s));

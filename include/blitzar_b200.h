@@ -226,6 +226,12 @@ void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, u
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
+/* Self-test of the binned bucket sort: sorts the (term, window) entries of the device-resident
+ * columns (window width `window_bits`, 0 = automatic) with the atomic and the binned path and returns
+ * the number of buckets whose end offset or entry multiset differs (0 = pass; ~0u when the binned path
+ * does not apply to the shape). */
+unsigned b200_selftest_sort(const struct sxt_sequence_descriptor* columns, unsigned num,
+                            unsigned window_bits);
 /* Per-launch CUDA-event timing of the dominant kernel (level-1 bucket accumulation) on the library
  * stream: enable, run, then read the total milliseconds and launch count since the last read. */
 void b200_profile_accumulate(int enable);
