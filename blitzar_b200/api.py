@@ -15,6 +15,8 @@ SXT_CPU_BACKEND, SXT_GPU_BACKEND = 1, 2
 SXT_CURVE_RISTRETTO255, SXT_CURVE_BLS_381, SXT_CURVE_BN_254, SXT_CURVE_GRUMPKIN = 0, 1, 2, 3
 # per curve: (projective ABI bytes, commitment-generator stride, commitment output bytes)
 CURVE_SIZES = {0: (160, 160, 32), 1: (144, 104, 48), 2: (96, 72, 72), 3: (96, 72, 72)}
+# bytes of one entry of the reference's partition tables (c21t / cg1t / cn1t / cgkt::compact_element)
+COMPACT_BYTES = {0: 120, 1: 96, 2: 64, 3: 64}
 
 SXT_SYMBOLS = [
     "sxt_init", "sxt_curve25519_compute_pedersen_commitments",
@@ -38,7 +40,8 @@ B200_SYMBOLS = [
     "b200_profile_read", "b200_set_reduce_groups", "b200_stream",
     "b200_synthetic_generators_device", "b200_commit_host_partials",
     "b200_fixed_msm_host_partials", "b200_multiexp_handle_new_device",
-    "b200_selftest_lane_arithmetic", "b200_selftest_sort",
+    "b200_selftest_lane_arithmetic", "b200_selftest_sort", "b200_partition_table_device",
+    "b200_multiexp_handle_write_partition_table",
 ]
 
 
@@ -178,6 +181,13 @@ class MultiexpHandle:
     def write_to_file(self, filename):
         lib().sxt_multiexp_handle_write_to_file(C.c_void_p(self.h), filename.encode())
 
+    def write_partition_table(self, filename, window_width=0):
+        """b200_multiexp_handle_write_partition_table: the reference's own handle file
+        ([u32 window_width][partition table]), readable by libblitzar's and this library's
+        sxt_multiexp_handle_new_from_file. window_width 0 = the reference's default."""
+        lib().b200_multiexp_handle_write_partition_table(C.c_void_p(self.h), filename.encode(),
+                                                         C.c_uint(window_width))
+
     def free(self):
         if self.h:
             lib().sxt_multiexp_handle_free(C.c_void_p(self.h))
@@ -287,6 +297,18 @@ def synthetic_generators_device(curve_id, out_ptr, n, first=0, projective=False)
     """b200_synthetic_generators_device: the reference benchmarks' generators, produced in HBM."""
     lib().b200_synthetic_generators_device(C.c_uint(curve_id), C.c_void_p(out_ptr), C.c_uint64(n),
                                            C.c_uint64(first), C.c_int(1 if projective else 0))
+
+
+def partition_table_bytes(curve_id, n, window_width):
+    """Size of the partition table of n generators (without the file's u32 header)."""
+    return -(-n // window_width) * (COMPACT_BYTES[curve_id] << window_width)
+
+
+def partition_table_device(curve_id, out_ptr, gens_ptr, n, window_width=0):
+    """b200_partition_table_device: the reference's partition table of n projective ABI generators
+    in HBM, written to out_ptr (partition_table_bytes). Enqueued on the library stream."""
+    lib().b200_partition_table_device(C.c_uint(curve_id), C.c_void_p(out_ptr), C.c_void_p(gens_ptr),
+                                      C.c_uint64(n), C.c_uint(window_width))
 
 
 def synthetic_generators(curve_id, n, first=0, projective=False):

@@ -783,6 +783,27 @@ void fixed_host(void* res, const HandleSet* hs, int mode, unsigned element_num_b
 
 const uint32_t kHandleMagic = 0x44483242u;  // "B2HD"
 
+// Window width of the reference's partition tables: 1..24, the range sxt_multiexp_handle_new_from_
+// file reads; 0 = the reference's default, BLITZAR_PARTITION_WINDOW_WIDTH or else 16
+// (mtxpp2::get_default_window_width, sxt/multiexp/pippenger2/window_width.cc).
+unsigned partition_window(unsigned w) {
+  if (w == 0) {
+    const char* env = std::getenv("BLITZAR_PARTITION_WINDOW_WIDTH");
+    w = env ? (unsigned)std::strtoul(env, nullptr, 10) : 16u;
+  }
+  B200_REQUIRE(w >= 1 && w <= 24, "partition table window width must be in 1..24");
+  return w;
+}
+// Groups per chunk of a partition-table build: 64 MiB of compact entries (at least one group), or
+// what BLITZAR_B200_PTABLE_CHUNK_BYTES allows (test hook: many chunks). The build's scratch
+// (projective points, denominators, inversion tree) is up to 2.6x the chunk's entries.
+uint64_t partition_chunk_groups(const CurveVTable& V, unsigned w) {
+  uint64_t bytes = 64ull << 20;
+  if (const char* env = std::getenv("BLITZAR_B200_PTABLE_CHUNK_BYTES"))
+    bytes = std::strtoull(env, nullptr, 10);
+  return std::max<uint64_t>(1, bytes / ((uint64_t)V.abi_compact_bytes << w));
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -1243,6 +1264,96 @@ void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, u
   require_init("b200_synthetic_generators_device");
   B200_REQUIRE(out_generators != nullptr, "out_generators == nullptr");
   vt(curve_id).synth_generators(ctx(), out_generators, n, first, projective != 0);
+}
+void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const void* generators_dev,
+                                 uint64_t n, unsigned window_width) {
+  std::lock_guard<std::mutex> lock(g_mutex);
+  require_init("b200_partition_table_device");
+  const CurveVTable& V = vt(curve_id);
+  const unsigned w = partition_window(window_width);
+  if (n == 0)
+    return;
+  B200_REQUIRE(out_table_dev != nullptr && generators_dev != nullptr,
+               "out_table_dev / generators_dev must not be null");
+  cudaStream_t s = g_state.stream;
+  DevBuf<unsigned char> gens(n * V.gen_bytes, s);
+  V.ingest_projective(ctx(), generators_dev, gens.p, n);
+  const uint64_t groups = (n + w - 1) / w, step = partition_chunk_groups(V, w);
+  const size_t group_bytes = (size_t)V.abi_compact_bytes << w;
+  for (uint64_t g = 0; g < groups; g += step)
+    V.partition_table(ctx(), gens.p, n, w, g, std::min(step, groups - g),
+                      static_cast<unsigned char*>(out_table_dev) + g * group_bytes);
+}
+// The handle's generators (window 0 of every shard's table, gathered in order on the primary
+// device) -> the reference's handle file, chunk by chunk: chunk i is built into device buffer i % 2
+// on the compute stream and copied into pinned host buffer i % 2 on the copy stream while the host
+// writes chunk i - 1 to the file.
+void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle* handle,
+                                                const char* filename, unsigned window_width) {
+  std::lock_guard<std::mutex> lock(g_mutex);
+  require_init("b200_multiexp_handle_write_partition_table");
+  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
+  B200_REQUIRE(h && filename, "null handle or filename");
+  const CurveVTable& V = vt(h->curve_id);
+  const unsigned w = partition_window(window_width);
+  cudaStream_t s = g_state.stream, sc = g_state.copy_stream;
+  DevBuf<unsigned char> gens((size_t)(h->n ? h->n : 1) * V.gen_bytes, s);
+  for (size_t p = 0; p < h->shards.size(); ++p) {
+    const int device = state_of(p).device;
+    const Handle* sh = h->shards[p];
+    unsigned char* dst = gens.p + (size_t)h->first[p] * V.gen_bytes;
+    const size_t bytes = (size_t)sh->n * V.gen_bytes;
+    if (device == g_state.device)
+      copy_d2d(dst, sh->gens, bytes, s);
+    else if (bytes)
+      B200_CUDA(cudaMemcpyPeerAsync(dst, g_state.device, sh->gens, device, bytes, s));
+  }
+  FILE* f = std::fopen(filename, "wb");
+  B200_REQUIRE(f != nullptr, "cannot open partition table file for writing");
+  const uint32_t hdr = w;  // in_memory_partition_table_accessor::write_to_file: [unsigned w][table]
+  B200_REQUIRE(std::fwrite(&hdr, sizeof(hdr), 1, f) == 1, "short write");
+  const uint64_t groups = (h->n + w - 1) / w;
+  const uint64_t step = std::min<uint64_t>(partition_chunk_groups(V, w), std::max<uint64_t>(groups, 1));
+  const size_t group_bytes = (size_t)V.abi_compact_bytes << w, chunk_bytes = step * group_bytes;
+  const uint64_t chunks = (groups + step - 1) / step;
+  B200_LOG(2, "partition table file: curve %u, n = %u, w = %u, %llu chunks of %llu groups",
+           h->curve_id, h->n, w, (unsigned long long)chunks, (unsigned long long)step);
+  DevBuf<unsigned char> dev0(chunks ? chunk_bytes : 1, s), dev1(chunks > 1 ? chunk_bytes : 1, s);
+  unsigned char* dev[2] = {dev0.p, dev1.p};
+  unsigned char* host[2] = {nullptr, nullptr};
+  cudaEvent_t built[2], copied[2];
+  for (int k = 0; k < 2; ++k) {
+    if (chunks > (uint64_t)k)
+      B200_CUDA(cudaHostAlloc((void**)&host[k], chunk_bytes, cudaHostAllocDefault));
+    B200_CUDA(cudaEventCreateWithFlags(&built[k], cudaEventDisableTiming));
+    B200_CUDA(cudaEventCreateWithFlags(&copied[k], cudaEventDisableTiming));
+  }
+  auto chunk_size = [&](uint64_t i) { return std::min(step, groups - i * step) * group_bytes; };
+  for (uint64_t i = 0; i <= chunks; ++i) {
+    if (i < chunks) {
+      const int k = (int)(i & 1);
+      if (i >= 2)  // dev[k] was last read by the copy of chunk i - 2
+        B200_CUDA(cudaStreamWaitEvent(s, copied[k], 0));
+      V.partition_table(ctx(), gens.p, h->n, w, i * step, std::min(step, groups - i * step), dev[k]);
+      B200_CUDA(cudaEventRecord(built[k], s));
+      B200_CUDA(cudaStreamWaitEvent(sc, built[k], 0));
+      copy_d2h(host[k], dev[k], chunk_size(i), sc);
+      B200_CUDA(cudaEventRecord(copied[k], sc));
+    }
+    if (i >= 1) {  // host[k] is refilled by chunk i + 1 only after this write
+      const int k = (int)((i - 1) & 1);
+      B200_CUDA(cudaEventSynchronize(copied[k]));
+      B200_REQUIRE(std::fwrite(host[k], chunk_size(i - 1), 1, f) == 1, "short write");
+    }
+  }
+  B200_REQUIRE(std::fclose(f) == 0, "short write");
+  stream_sync(s);
+  for (int k = 0; k < 2; ++k) {
+    if (host[k])
+      B200_CUDA(cudaFreeHost(host[k]));
+    B200_CUDA(cudaEventDestroy(built[k]));
+    B200_CUDA(cudaEventDestroy(copied[k]));
+  }
 }
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   std::lock_guard<std::mutex> lock(g_mutex);

@@ -264,6 +264,18 @@ struct Ed25519 {
     F::from_radix51(p.T, s + 10);
     point_to_gen(g, p);
   }
+  // the inverse of load_compact_abi for the point p with zi = 1 / Z: canonical radix-2^51 limbs
+  // (each < 2^51, value < p) of x = X zi, y = Y zi and T = x y
+  static B200_HD void store_compact_abi(void* dst, const Point& p, const fe& zi) {
+    u64* d = (u64*)dst;
+    fe x, y, t;
+    F::mul(x, p.X, zi);
+    F::mul(y, p.Y, zi);
+    F::mul(t, x, y);
+    F::to_radix51(d, x);
+    F::to_radix51(d + 5, y);
+    F::to_radix51(d + 10, t);
+  }
   static B200_HD void store_proj_abi(void* dst, const Point& p) {
     u64* d = (u64*)dst;
     F::to_radix51(d, p.X);
@@ -628,6 +640,23 @@ template <class FieldT, class CP> struct Weierstrass {
     }
     F::load(g.x, s);
     F::load(g.y, s + N);
+  }
+  // the inverse of load_compact_abi for the point p with zi = 1 / Z (anything when Z = 0): the
+  // affine Montgomery limbs, or the identity {X = {0, .., 0, ~0}, Y = R mod p}
+  // (compact_element::identity(), sxt/curve_bng1/type/compact_element.h:32-37)
+  static B200_HD void store_compact_abi(void* dst, const Point& p, const fe& zi) {
+    u32* d = (u32*)dst;
+    fe x, y;
+    if (F::is_zero(p.Z)) {
+      x = F::zero();
+      x.l[N - 2] = x.l[N - 1] = 0xffffffffu;
+      y = F::one();
+    } else {
+      F::mul(x, p.X, zi);
+      F::mul(y, p.Y, zi);
+    }
+    F::store(d, x);
+    F::store(d + N, y);
   }
   // projective ABI struct {X,Y,Z} -> affine generator (one field inversion)
   static B200_HD void load_proj_abi(Gen& g, const void* src) {

@@ -8,6 +8,7 @@
 
 #include "engine_api.cuh"
 #include "msm.cuh"
+#include "ptable.cuh"
 #include "synth.cuh"
 
 namespace b200 {
@@ -285,6 +286,11 @@ template <class C> struct CurveOps {
                                bool projective) {
     Synth<C>::generators(ctx.s, out_dev, n, first, projective);
   }
+  static void partition_table(const EngineCtx& ctx, const void* gens, uint64_t n, unsigned w,
+                              uint64_t first_group, uint64_t groups, void* out_dev) {
+    build_partition_table<C>(ctx.s, (const Gen*)gens, n, w, first_group, groups,
+                             (unsigned char*)out_dev);
+  }
 };
 
 #define B200_DEFINE_CURVE_VTABLE(NAME, C)                                                          \
@@ -303,6 +309,7 @@ template <class C> struct CurveOps {
                             &CurveOps<C>::synth_generators,                                        \
                             (unsigned)C::kAbiCompactBytes,                                         \
                             &CurveOps<C>::ingest_compact_table,                                    \
-                            &CurveOps<C>::build_table}
+                            &CurveOps<C>::build_table,                                             \
+                            &CurveOps<C>::partition_table}
 
 }  // namespace b200

@@ -131,6 +131,10 @@ struct CurveVTable {
   // fills windows 1 .. windows-1 of a fixed-base table whose window 0 (n generators) is in place
   void (*build_table)(const EngineCtx&, void* table, uint64_t n, unsigned window_bits,
                       unsigned windows);
+  // groups [first_group, first_group + groups) of the reference's partition table of width w over n
+  // generators (device generator layout; ptable.cuh) -> compact ABI entries at out_dev
+  void (*partition_table)(const EngineCtx&, const void* gens, uint64_t n, unsigned w,
+                          uint64_t first_group, uint64_t groups, void* out_dev);
 };
 extern const CurveVTable kVTableEd25519, kVTableBls12381, kVTableBn254, kVTableGrumpkin;
 

@@ -433,6 +433,8 @@ struct F25519 {
     sqr_n(t, t, 5);
     mul(r, t, a11);
   }
+  // the name the top of the batch-inversion tree calls (batch_affine.cuh); here the Fermat ladder
+  static B200_HD void invert_eea(E& r, const E& a) { invert(r, a); }
   // a^((p-5)/8) = a^(2^252 - 3): (2^250-1) << 2 | 1
   static B200_HD void pow22523(E& r, const E& a) {
     E t, a11;

@@ -222,6 +222,17 @@ void b200_combine_partials_projective_device(unsigned curve_id, void* out_res,
  * *_p2 structs (projective != 0, handle input) or affine structs at the commitment stride. */
 void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, uint64_t n,
                                       uint64_t first, int projective);
+/* The reference's partition table (2^w compact elements per group of w generators, identity-padded)
+ * of n projective ABI generators already in HBM, written to out_table_dev (device, 2^w * ceil(n/w) *
+ * compact bytes). window_width 1..24; 0 = the reference's default (BLITZAR_PARTITION_WINDOW_WIDTH,
+ * else 16). Enqueued on the library stream; returns without synchronising. */
+void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const void* generators_dev,
+                                 uint64_t n, unsigned window_width);
+/* Writes the handle as the reference's handle file ([u32 window_width][table],
+ * in_memory_partition_table_accessor.h:98-105), readable by libblitzar's
+ * sxt_multiexp_handle_new_from_file and by this library's. Synchronises before returning. */
+void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle* handle,
+                                                const char* filename, unsigned window_width);
 /* Self-test of the warp-cooperative (lane-sliced) field arithmetic of the tail kernels against the
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
