@@ -324,4 +324,71 @@ struct FinalEntriesBody {
   }
 };
 
+template <class C> struct WalkInput {  // what the chunk walk (msm.cuh) sums
+  const typename C::Gen* gens;
+  const u64* entries;  // (key << 32) | (index into gens << 1) | negate
+  const u32* m_ptr;    // number of entries (device)
+  u64 m_max;           // bound on *m_ptr
+};
+
+// L pair levels over the sorted, padded level-0 entries (d_m[0] of slots_max slots). Returns the walk
+// over the last level's points (count in d_m[9]); its gens and entries are the caller's to free.
+template <class C>
+WalkInput<C> run_pair_levels(stream_t s, u32 L, const u64* entries, const typename C::Gen* gens,
+                             u32* d_m, u64 slots_max, u32 pair_batch) {
+  typedef typename C::F F;
+  typedef typename F::E fe;
+  typedef typename C::Gen Gen;
+  // pairs per thread halve from level to level (a thread's sums are its own next-level inputs)
+  u32 B = pair_batch ? pair_batch : 32u;
+  while (B < (1u << L))
+    B *= 2;
+  B = (B >> (L - 1)) << (L - 1);
+  const u64 T = ((slots_max >> 1) + B - 1) / B;  // the same threads at every level
+  // The level is cut in two halves of threads (A, B) on two streams. The heavy passes are chained
+  // A, B, A, B, ... by events, so the inversion tree of one half (a chain of small latency-bound
+  // kernels ending in one Fermat inversion) runs under the heavy pass of the other half instead
+  // of leaving the GPU idle once per level. A thread's next-level inputs are its own outputs, so
+  // the halves never read each other's data.
+  stream_t s2 = aux_stream();
+  const u64 Ta = T / 2, Tb = T - Ta;
+  const Gen* in = nullptr;
+  fe* pre = (fe*)dev_alloc((slots_max >> 1) * sizeof(fe), s);
+  fe* totals = (fe*)dev_alloc(T * sizeof(fe), s);
+  std::vector<void*> level_bufs = {pre, totals};
+  const PairLevel<C> lv0{entries, gens, nullptr, d_m, 0, B};
+  launch(PairPass1Body<C>{lv0, pre, totals, 0}, Ta, s);
+  stream_follow(s2, s);
+  launch(PairPass1Body<C>{lv0, pre, totals, Ta}, Tb, s2);
+  for (u32 l = 0; l < L; ++l) {
+    const u64 npairs = slots_max >> (l + 1);
+    const bool last = l + 1 == L;
+    // buffers of the next level come from the main stream's pool; the second stream touches
+    // them only after following the main stream past this point
+    Gen* out = (Gen*)dev_alloc(npairs * sizeof(Gen), s);
+    fe* pre_next = last ? nullptr : (fe*)dev_alloc((npairs >> 1) * sizeof(fe), s);
+    fe* totals_next = last ? nullptr : (fe*)dev_alloc(T * sizeof(fe), s);
+    level_bufs.insert(level_bufs.end(), {out, pre_next, totals_next});  // null on the last level
+    PairLevel<C> lv{l == 0 ? entries : nullptr, l == 0 ? gens : nullptr, in, d_m, l, B >> l};
+    const u32 desc = (l & 1u) ? 0u : 1u;
+    batch_invert<F>(s, totals, Ta);
+    stream_follow(s, s2);  // after the other half's previous heavy pass
+    launch(PairPass2Body<C>{lv, pre, totals, out, pre_next, totals_next, desc, 0}, Ta, s);
+    batch_invert<F>(s2, totals + Ta, Tb);
+    stream_follow(s2, s);
+    launch(PairPass2Body<C>{lv, pre, totals, out, pre_next, totals_next, desc, Ta}, Tb, s2);
+    in = out;
+    pre = pre_next;
+    totals = totals_next;
+  }
+  stream_follow(s, s2);  // the level buffers are freed on s after s2's last pass has read them
+  for (void* ptr : level_bufs)
+    if (ptr != (void*)in)  // the last level's points feed the chunk walk (freed by the caller)
+      dev_free(ptr, s);
+  const u64 m_max = slots_max >> L;
+  u64* entries_l = (u64*)dev_alloc(m_max * sizeof(u64), s);
+  launch(FinalEntriesBody{entries, d_m, L, entries_l, d_m + 9}, m_max, s);
+  return {in, entries_l, d_m + 9, m_max};
+}
+
 }  // namespace b200

@@ -303,8 +303,8 @@ inline void exclusive_scan(u32* data, u64 n, stream_t s, u32 chunk = kScanChunkF
 #if defined(__CUDACC__) && !defined(B200_EMULATE)
 #define B200_BINNED_SORT 1
 // ---- binned sort of the (term, window) entries (block-cooperative, CUDA only) ----------------------
-// The same output as CountBody -> exclusive_scan -> ScatterBody (entries sorted by key, counts[k] = END
-// offset of bucket k, d_m[0] = M) without a global atomic or a scattered 8-byte store per entry:
+// The same unpadded SortedLayout as CountBody -> exclusive_scan -> ScatterBody (sort_entries) without a
+// global atomic or a scattered 8-byte store per entry:
 //   1. MicroCountBody: per tile of terms, a shared-memory histogram of micro-bins (key >> shift),
 //      flushed with one global atomic per non-zero counter
 //   2. PlanBinsBody: one block scans the micro-bins and groups consecutive ones into bins of at most
@@ -1169,46 +1169,123 @@ inline MsmPlan msm_make_plan(std::vector<ColumnDesc> cols, const MsmOptions& opt
   return p;
 }
 
-// Sorts the entries of `cols` (host descriptors over device scalars, window width c; 0 = automatic)
-// with the atomic path and with the binned path, and returns the number of buckets whose end offset
-// or entry multiset differs between the two (0 = agree; ~0u when the binned path does not apply).
-inline unsigned sort_selftest(stream_t s, std::vector<ColumnDesc> cols, u32 c) {
+// The columns of a plan restricted to the terms [begin, end), staged with one H2D as a block
+// [ColumnDesc x ncols][u64 x (ncols+1)]: descriptors, then the prefix of their lengths.
+struct StagedRange {
+  const ColumnDesc* d_cols = nullptr;  // the block; null when the range holds no term
+  const u64* d_col_start = nullptr;
+  u64 total_terms = 0, max_entries = 0;
+  u32 max_windows = 0;  // windows of the widest non-empty column
+  StagedRange(stream_t s, const MsmPlan& plan, u64 begin, u64 end) {
+    const u32 ncols = plan.ncols;
+    std::vector<ColumnDesc> cols(plan.cols);
+    std::vector<u64> col_start(ncols + 1, 0);
+    for (u32 j = 0; j < ncols; ++j) {
+      u64 lo = std::min<u64>(begin, cols[j].n), hi = std::min<u64>(end, cols[j].n);
+      cols[j].base += lo * cols[j].row_stride;
+      cols[j].n = (u32)(hi - lo);
+      col_start[j + 1] = col_start[j] + cols[j].n;
+      max_entries += (u64)cols[j].n * cols[j].num_windows;
+      max_windows = std::max(max_windows, cols[j].n ? cols[j].num_windows : 0u);
+    }
+    total_terms = col_start[ncols];
+    if (total_terms == 0)
+      return;
+    B200_REQUIRE(max_entries < (1ull << 32) && end - begin < (1ull << 31),
+                 "too many (term, window) entries for one sort pass");
+    const size_t desc_bytes = ncols * sizeof(ColumnDesc), start_bytes = (ncols + 1) * sizeof(u64);
+    std::vector<unsigned char> stage(desc_bytes + start_bytes);
+    std::memcpy(stage.data(), cols.data(), desc_bytes);
+    std::memcpy(stage.data() + desc_bytes, col_start.data(), start_bytes);
+    d_cols = (const ColumnDesc*)stage_to_device(s, stage.data(), stage.size());
+    d_col_start = (const u64*)((const unsigned char*)d_cols + desc_bytes);
+  }
+};
+
+struct SortedLayout {  // the sorted (term, window) entries of one range, read by every later stage
+  u64* entries;   // sorted by key, (key << 32) | (generator index << 1) | negate; with L > 0 every
+                  // bucket is followed by pad entries (index kPadIndex) up to a multiple of 2^L slots
+  u32* counts;    // [nkeys + 1]: counts[k] = END offset of bucket k's real entries
+  u32* starts;    // [nkeys + 1]: padded start offset of every bucket; null when L = 0
+  u32* d_m;       // [16]: d_m[0] = number of slots; the rest is scratch of the later stages
+  u64 slots_max;  // slots allocated for `entries` (bound on d_m[0])
+  bool binned;    // sorted by the binned path
+};
+
+// Sorts a staged range into a SortedLayout and flags window_used[w] for every window with an entry.
+// The binned sort (CUDA build) serves unpadded layouts (L = 0) of at most kMicroBins << kMaxBinShift
+// keys: always with opt.sort_path 2, from kBinnedSortMinEntries entries on with 1. The atomic count +
+// scan + scatter sorts every other case.
+inline SortedLayout sort_entries(stream_t s, const MsmPlan& plan, const StagedRange& r, u32 L,
+                                 const MsmOptions& opt, u32* window_used) {
+  const u32 ncols = plan.ncols, c = plan.c, nbuckets = plan.nbuckets;
+  const u64 nkeys = plan.nkeys, max_entries = r.max_entries, total_terms = r.total_terms;
+  SortedLayout out{};
+  out.slots_max = L ? ((max_entries + nkeys * ((1ull << L) - 1) + (1ull << L) - 1) >> L) << L : max_entries;
+  out.counts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
+  out.d_m = (u32*)dev_alloc(16 * sizeof(u32), s);
+  out.entries = (u64*)dev_alloc(out.slots_max * sizeof(u64), s);
 #ifdef B200_BINNED_SORT
+  out.binned = L == 0 && opt.sort_path != 0 && binned_sort_shift(nkeys) <= kMaxBinShift &&
+               (opt.sort_path == 2 || max_entries >= kBinnedSortMinEntries);
+  if (out.binned)
+    binned_sort(s, r.d_cols, r.d_col_start, ncols, c, nbuckets, total_terms, max_entries,
+                r.max_windows, nkeys, out.entries, out.counts, out.d_m);
+#endif
+  if (!out.binned) {
+    dev_zero(out.counts, (nkeys + 1) * sizeof(u32), s);
+    launch(CountBody{r.d_cols, r.d_col_start, ncols, c, nbuckets, out.counts}, total_terms, s);
+    if (L) {
+      launch(WindowUsedFromCountsBody{out.counts, nkeys, nbuckets, window_used}, (nkeys + 255) / 256, s);
+      launch(PadCountsBody{out.counts, (1u << L) - 1u}, nkeys, s);
+    }
+    exclusive_scan(out.counts, nkeys + 1, s);  // counts[nkeys] = number of (padded) entries
+    copy_d2d(out.d_m, out.counts + nkeys, sizeof(u32), s);
+    if (L) {
+      out.starts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
+      copy_d2d(out.starts, out.counts, (nkeys + 1) * sizeof(u32), s);
+    }
+    const bool window_major = opt.scatter_window_major && r.max_windows > 1;
+    launch(ScatterBody{r.d_cols, r.d_col_start, ncols, c, nbuckets, out.counts, out.entries,
+                       window_major ? total_terms : 0},
+           window_major ? total_terms * r.max_windows : total_terms, s);
+  }
+  if (L)
+    launch(FillPadsBody{out.starts, out.counts, out.entries}, nkeys, s);
+  else
+    launch(WindowUsedBody{out.counts, nbuckets, window_used}, plan.total_windows, s);
+  return out;
+}
+
+// Sorts `cols` (host descriptors over device scalars, window width c; 0 = automatic) with sort_entries
+// forced to the atomic and to the binned path and returns the number of buckets whose end offset or
+// entry multiset differs between the two (0 = agree; ~0u when the binned path does not apply).
+inline unsigned sort_selftest(stream_t s, std::vector<ColumnDesc> cols, u32 c) {
   MsmOptions opt;
   opt.window_bits = c;
   const MsmPlan plan = msm_make_plan(std::move(cols), opt, 160);
-  if (plan.total_terms == 0 || binned_sort_shift(plan.nkeys) > kMaxBinShift)
+  const StagedRange r(s, plan, 0, plan.max_n);
+  if (r.total_terms == 0)
     return ~0u;
-  const u32 ncols = plan.ncols;
-  const u64 nkeys = plan.nkeys, M = plan.total_entries;
-  std::vector<u64> col_start(ncols + 1, 0);
-  for (u32 j = 0; j < ncols; ++j)
-    col_start[j + 1] = col_start[j] + plan.cols[j].n;
-  DevBuf<ColumnDesc> d_cols(ncols, s);
-  DevBuf<u64> d_col_start(ncols + 1, s);
-  copy_h2d(d_cols.p, plan.cols.data(), ncols * sizeof(ColumnDesc), s);
-  copy_h2d(d_col_start.p, col_start.data(), (ncols + 1) * sizeof(u64), s);
-  DevBuf<u32> counts_a(nkeys + 1, s), counts_b(nkeys + 1, s), d_m(16, s);
-  DevBuf<u64> entries_a(M + 1, s), entries_b(M + 1, s);
-  dev_zero(counts_a.p, (nkeys + 1) * sizeof(u32), s);
-  launch(CountBody{d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, counts_a.p},
-         plan.total_terms, s);
-  exclusive_scan(counts_a.p, nkeys + 1, s);
-  launch(ScatterBody{d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, counts_a.p, entries_a.p, 0},
-         plan.total_terms, s);
-  u32 max_windows = 0;
-  for (const auto& col : plan.cols)
-    max_windows = std::max(max_windows, col.n ? col.num_windows : 0u);
-  binned_sort(s, d_cols.p, d_col_start.p, ncols, plan.c, plan.nbuckets, plan.total_terms, M,
-              max_windows, nkeys, entries_b.p, counts_b.p, d_m.p);
+  const u64 nkeys = plan.nkeys, M = r.max_entries;
+  DevBuf<u32> window_used(plan.total_windows, s);  // not compared: both paths set it from the counts
+  opt.sort_path = 0;
+  const SortedLayout a = sort_entries(s, plan, r, 0, opt, window_used.p);
+  opt.sort_path = 2;
+  const SortedLayout b = sort_entries(s, plan, r, 0, opt, window_used.p);
   std::vector<u32> ca(nkeys + 1), cb(nkeys + 1), m(1);
   std::vector<u64> ea(M), eb(M);
-  copy_d2h(ca.data(), counts_a.p, (nkeys + 1) * sizeof(u32), s);
-  copy_d2h(cb.data(), counts_b.p, (nkeys + 1) * sizeof(u32), s);
-  copy_d2h(m.data(), d_m.p, sizeof(u32), s);
-  copy_d2h(ea.data(), entries_a.p, M * sizeof(u64), s);
-  copy_d2h(eb.data(), entries_b.p, M * sizeof(u64), s);
+  copy_d2h(ca.data(), a.counts, (nkeys + 1) * sizeof(u32), s);
+  copy_d2h(cb.data(), b.counts, (nkeys + 1) * sizeof(u32), s);
+  copy_d2h(m.data(), b.d_m, sizeof(u32), s);
+  copy_d2h(ea.data(), a.entries, M * sizeof(u64), s);
+  copy_d2h(eb.data(), b.entries, M * sizeof(u64), s);
   stream_sync(s);
+  for (void* p : {(void*)a.entries, (void*)a.counts, (void*)a.d_m, (void*)b.entries, (void*)b.counts,
+                  (void*)b.d_m, (void*)r.d_cols})
+    dev_free(p, s);
+  if (!b.binned)
+    return ~0u;
   unsigned bad = m[0] == ca[nkeys] ? 0u : 1u;  // M: counts[nkeys] of the atomic path
   for (u64 k = 0; k < nkeys; ++k) {
     const u32 lo = k ? ca[k - 1] : 0u, hi = ca[k];
@@ -1222,12 +1299,6 @@ inline unsigned sort_selftest(stream_t s, std::vector<ColumnDesc> cols, u32 c) {
       ++bad;
   }
   return bad;
-#else
-  (void)s;
-  (void)cols;
-  (void)c;
-  return ~0u;
-#endif
 }
 
 // Optional per-range hook: called before the terms [begin, end) are touched (the C-ABI layer uses
@@ -1240,6 +1311,64 @@ struct RangeHook {
   virtual ~RangeHook() {}
 };
 
+// Chunk walk of `walk` into `target`, then the cascade over its pieces (appended to to_free) on `tail`
+// when it differs from s. Returns the stream of the last level.
+template <class C>
+stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, u32 unit_z,
+                    typename C::Point* target, const MsmOptions& opt, std::vector<void*>& to_free) {
+  typedef typename C::Point Point;
+  // a chunk of K entries leaves 2 pieces, so K must exceed 2 for the cascade to shrink
+  // at C2, K = 64 trims the cascade more than it costs the first level
+  u32 K = opt.chunk1 ? std::max(opt.chunk1, 4u) : (walk.m_max >= (1ull << 23) ? 64u : 32u);
+  const u32 chunkn = std::max(opt.chunkn, 4u);
+  const u32* lvl_keys = nullptr;
+  const Point* lvl_pieces = nullptr;
+  stream_t cs = s;  // stream of the current cascade level
+  for (int level = 0;; ++level) {
+    const bool final_level = walk.m_max <= K;
+    u64 T = (walk.m_max + K - 1) / K;
+    u32* out_keys = final_level ? nullptr : (u32*)dev_alloc(2 * T * sizeof(u32), cs);
+    Point* out_pieces = final_level ? nullptr : (Point*)dev_alloc(2 * T * sizeof(Point), cs);
+    to_free.insert(to_free.end(), {out_keys, out_pieces});
+    u32* out_m = d_m + 1 + (level % 8);
+    if (level == 0) {
+      // faster on ed25519 (a run start is a multiplication by a constant there); the Weierstrass
+      // start is free, so the extra addition loses
+      const bool uniform =
+          opt.uniform_add == 2 ? C::kCurveId == kRistretto255 : opt.uniform_add != 0;
+      if (uniform)
+        launch(AccumulateBody<C, true, SeqExec, true>{nullptr, walk.entries, walk.gens, nullptr,
+                                                      walk.m_ptr, K, final_level, target, out_keys,
+                                                      out_pieces, out_m, unit_z},
+               T, s);
+      else
+        launch(AccumulateBody<C, true>{nullptr, walk.entries, walk.gens, nullptr, walk.m_ptr, K,
+                                       final_level, target, out_keys, out_pieces, out_m, unit_z},
+               T, s);
+      KernelTimer::get().end(s);
+      if (tail != s)
+        stream_follow(tail, s);
+      cs = tail;
+    } else if (T <= opt.quad_threshold) {
+      launch(AccumulateBody<C, false, QuadExec>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr,
+                                                K, final_level, target, out_keys, out_pieces, out_m, 0u},
+             T * QuadExec::kLanes, cs);
+    } else {
+      launch(AccumulateBody<C, false>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr, K,
+                                      final_level, target, out_keys, out_pieces, out_m, 0u},
+             T, cs);
+    }
+    if (final_level)
+      break;
+    lvl_keys = out_keys;
+    lvl_pieces = out_pieces;
+    walk.m_ptr = out_m;
+    walk.m_max = 2 * T;
+    K = chunkn;
+  }
+  return cs;
+}
+
 // Sort + accumulate the terms [begin, end) of every column into d_buckets (indexed by the plan's
 // keys). gens[i] pairs with term i (absolute index). add_into: buckets already hold the sums of
 // earlier ranges (this range then goes through a scratch bucket array + MergeBucketsBody). Enqueued on
@@ -1251,37 +1380,12 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
                           u64 end, bool add_into, typename C::Point* d_buckets,
                           u32* d_window_used, const MsmOptions& opt, stream_t tail,
                           RangeHook* hook = nullptr) {
-  typedef typename C::Point Point;
-  const u32 ncols = plan.ncols;
-  std::vector<ColumnDesc> cols(plan.cols);
-  std::vector<u64> col_start(ncols + 1, 0);
-  u64 max_entries = 0;
-  for (u32 j = 0; j < ncols; ++j) {
-    u64 lo = std::min<u64>(begin, cols[j].n), hi = std::min<u64>(end, cols[j].n);
-    cols[j].base += lo * cols[j].row_stride;
-    cols[j].n = (u32)(hi - lo);
-    col_start[j + 1] = col_start[j] + cols[j].n;
-    max_entries += (u64)cols[j].n * cols[j].num_windows;
-  }
-  const u64 total_terms = col_start[ncols];
-  if (total_terms == 0)
+  const StagedRange r(s, plan, begin, end);
+  if (r.total_terms == 0)
     return;
-  B200_REQUIRE(max_entries < (1ull << 32) && end - begin < (1ull << 31),
-               "too many (term, window) entries for one sort pass");
-  const u32 c = plan.c, nbuckets = plan.nbuckets;
-  const u64 nkeys = plan.nkeys;
   gens += begin;  // entry indices are relative to the range
-
-  // one staging block: [ColumnDesc x ncols][u64 x (ncols+1)], copied with a single H2D
-  const size_t desc_bytes = ncols * sizeof(ColumnDesc), start_bytes = (ncols + 1) * sizeof(u64);
-  std::vector<unsigned char> stage(desc_bytes + start_bytes);
-  std::memcpy(stage.data(), cols.data(), desc_bytes);
-  std::memcpy(stage.data() + desc_bytes, col_start.data(), start_bytes);
-  unsigned char* d_stage = (unsigned char*)stage_to_device(s, stage.data(), stage.size());
-  const ColumnDesc* d_cols = (const ColumnDesc*)d_stage;
-  const u64* d_col_start = (const u64*)(d_stage + desc_bytes);
-
   StageRange nvtx_sort("msm: digit count + scan + scatter");
+  const u64 max_entries = r.max_entries, nkeys = plan.nkeys;
   // Batch-affine pair levels (short Weierstrass curves, large passes): L levels, buckets padded to
   // multiples of 2^L slots; L from the mean bucket load so that pads stay below ~1/4 of the slots.
   u32 L = 0;
@@ -1295,211 +1399,39 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
     while (L > 0 && max_entries + nkeys * ((1ull << L) - 1) >= (1ull << 32) - (1ull << L))
       --L;
   }
-  const u64 slots_max =
-      L ? ((max_entries + nkeys * ((1ull << L) - 1) + (1ull << L) - 1) >> L) << L : max_entries;
-  u32* d_counts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
-  u32* d_m = (u32*)dev_alloc(16 * sizeof(u32), s);
-  u64* d_entries = (u64*)dev_alloc(slots_max * sizeof(u64), s);
-  u32* d_starts = nullptr;
-  u32 max_windows = 0;
-  for (u32 j = 0; j < ncols; ++j)
-    max_windows = std::max(max_windows, cols[j].n ? cols[j].num_windows : 0u);
-  bool binned = false;
-#ifdef B200_BINNED_SORT
-  binned = L == 0 && opt.sort_path != 0 && binned_sort_shift(nkeys) <= kMaxBinShift &&
-           (opt.sort_path == 2 || max_entries >= kBinnedSortMinEntries);
-#endif
-  if (binned) {
-#ifdef B200_BINNED_SORT
-    binned_sort(s, d_cols, d_col_start, ncols, c, nbuckets, total_terms, max_entries, max_windows,
-                nkeys, d_entries, d_counts, d_m);
-#endif
-  } else {
-    dev_zero(d_counts, (nkeys + 1) * sizeof(u32), s);
-    launch(CountBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts}, total_terms, s);
-  }
-  if (L) {
-    launch(WindowUsedFromCountsBody{d_counts, nkeys, nbuckets, d_window_used}, (nkeys + 255) / 256, s);
-    launch(PadCountsBody{d_counts, (1u << L) - 1u}, nkeys, s);
-  }
-  if (!binned) {
-    exclusive_scan(d_counts, nkeys + 1, s);  // d_counts[nkeys] = number of (padded) entries
-    copy_d2d(d_m, d_counts + nkeys, sizeof(u32), s);
-    if (L) {
-      d_starts = (u32*)dev_alloc((nkeys + 1) * sizeof(u32), s);
-      copy_d2d(d_starts, d_counts, (nkeys + 1) * sizeof(u32), s);
-    }
-    if (opt.scatter_window_major && max_windows > 1)
-      launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, total_terms},
-             total_terms * max_windows, s);
-    else
-      launch(ScatterBody{d_cols, d_col_start, ncols, c, nbuckets, d_counts, d_entries, 0},
-             total_terms, s);
-  }
-  // d_counts[k] is now the END offset of bucket k's real entries
-  if (L)
-    launch(FillPadsBody{d_starts, d_counts, d_entries}, nkeys, s);
-  else
-    launch(WindowUsedBody{d_counts, nbuckets, d_window_used}, plan.total_windows, s);
-
+  const SortedLayout sorted = sort_entries(s, plan, r, L, opt, d_window_used);
   B200_LOG(3, "range [%llu, %llu): %llu terms, %llu entries max, c=%u, %llu keys, pair levels %u",
-           (unsigned long long)begin, (unsigned long long)end, (unsigned long long)total_terms,
-           (unsigned long long)max_entries, c, (unsigned long long)nkeys, L);
+           (unsigned long long)begin, (unsigned long long)end, (unsigned long long)r.total_terms,
+           (unsigned long long)max_entries, plan.c, (unsigned long long)nkeys, L);
+  WalkInput<C> walk{gens, sorted.entries, sorted.d_m, max_entries};
   std::vector<void*> to_free;
-  const typename C::Gen* walk_gens = gens;
-  const u64* walk_entries = d_entries;
-  u64 m_max = max_entries;
-  u32* m_ptr = d_m;
   if (hook)
     hook->before_accumulate();
   KernelTimer::get().begin(s);
   StageRange nvtx_acc("msm: bucket accumulation");
   if constexpr (C::kBatchAffine) {
     if (L) {
-      typedef typename C::F F;
-      typedef typename F::E fe;
-      typedef typename C::Gen Gen;
-      // pairs per thread halve from level to level (a thread's sums are its own next-level inputs)
-      u32 B = opt.pair_batch ? opt.pair_batch : 32u;
-      while (B < (1u << L))
-        B *= 2;
-      B = (B >> (L - 1)) << (L - 1);
-      const u64 T = ((slots_max >> 1) + B - 1) / B;  // the same threads at every level
-      // The level is cut in two halves of threads (A, B) on two streams. The heavy passes are chained
-      // A, B, A, B, ... by events, so the inversion tree of one half (a chain of small latency-bound
-      // kernels ending in one Fermat inversion) runs under the heavy pass of the other half instead
-      // of leaving the GPU idle once per level. A thread's next-level inputs are its own outputs, so
-      // the halves never read each other's data.
-      stream_t s2 = aux_stream();
-      const u64 Ta = T / 2, Tb = T - Ta;
-      const Gen* in = nullptr;
-      fe* pre = (fe*)dev_alloc((slots_max >> 1) * sizeof(fe), s);
-      fe* totals = (fe*)dev_alloc(T * sizeof(fe), s);
-      std::vector<void*> level_bufs = {pre, totals};
-      {
-        PairLevel<C> lv0{d_entries, gens, nullptr, d_m, 0, B};
-        launch(PairPass1Body<C>{lv0, pre, totals, 0}, Ta, s);
-        stream_follow(s2, s);
-        launch(PairPass1Body<C>{lv0, pre, totals, Ta}, Tb, s2);
-      }
-      for (u32 l = 0; l < L; ++l) {
-        const u64 npairs = slots_max >> (l + 1);
-        const bool last = l + 1 == L;
-        // buffers of the next level come from the main stream's pool; the second stream touches
-        // them only after following the main stream past this point
-        Gen* out = (Gen*)dev_alloc(npairs * sizeof(Gen), s);
-        fe* pre_next = last ? nullptr : (fe*)dev_alloc((npairs >> 1) * sizeof(fe), s);
-        fe* totals_next = last ? nullptr : (fe*)dev_alloc(T * sizeof(fe), s);
-        level_bufs.push_back(out);
-        if (!last) {
-          level_bufs.push_back(pre_next);
-          level_bufs.push_back(totals_next);
-        }
-        PairLevel<C> lv{l == 0 ? d_entries : nullptr, l == 0 ? gens : nullptr, in, d_m, l, B >> l};
-        const u32 desc = (l & 1u) ? 0u : 1u;
-        batch_invert<F>(s, totals, Ta);
-        stream_follow(s, s2);  // after the other half's previous heavy pass
-        launch(PairPass2Body<C>{lv, pre, totals, out, pre_next, totals_next, desc, 0}, Ta, s);
-        batch_invert<F>(s2, totals + Ta, Tb);
-        stream_follow(s2, s);
-        launch(PairPass2Body<C>{lv, pre, totals, out, pre_next, totals_next, desc, Ta}, Tb, s2);
-        in = out;
-        pre = pre_next;
-        totals = totals_next;
-      }
-      stream_follow(s, s2);
-      level_bufs.pop_back();  // the last level's points feed the chunk walk (freed with to_free)
-      for (void* ptr : level_bufs)
-        if (ptr != (void*)in)
-          dev_free(ptr, s);
-      m_max = slots_max >> L;
-      u64* entries_l = (u64*)dev_alloc(m_max * sizeof(u64), s);
-      launch(FinalEntriesBody{d_entries, d_m, L, entries_l, d_m + 9}, m_max, s);
-      to_free.push_back((void*)in);
-      to_free.push_back(entries_l);
-      walk_gens = in;
-      walk_entries = entries_l;
-      m_ptr = d_m + 9;
+      walk = run_pair_levels<C>(s, L, sorted.entries, gens, sorted.d_m, sorted.slots_max,
+                                opt.pair_batch);
+      to_free = {(void*)walk.gens, (void*)walk.entries};
     }
   }
-
-  // a chunk of K entries leaves 2 pieces, so K must exceed 2 for the cascade to shrink
-  // at C2, K = 64 trims the cascade more than it costs the first level
-  const u32 chunk1_auto = m_max >= (1ull << 23) ? 64u : 32u;
-  const u32 chunk1 = opt.chunk1 == 0 ? chunk1_auto : (opt.chunk1 < 4 ? 4u : opt.chunk1);
-  const u32 chunkn = opt.chunkn < 4 ? 4u : opt.chunkn;
-  Point* d_target = d_buckets;
-  if (add_into)  // later ranges: own bucket array, merged into the shared one below
-    d_target = (Point*)dev_alloc(nkeys * sizeof(Point), s);
-  u32 K = chunk1;
-  const u32* lvl_keys = nullptr;
-  const Point* lvl_pieces = nullptr;
-  bool first = true;
-  int level = 0;
-  stream_t cs = s;  // stream of the current cascade level
-  for (;;) {
-    bool final_level = m_max <= K;
-    u64 T = (m_max + K - 1) / K;
-    u32* out_keys = nullptr;
-    Point* out_pieces = nullptr;
-    u32* out_m = d_m + 1 + (level % 8);
-    if (!final_level) {
-      out_keys = (u32*)dev_alloc(2 * T * sizeof(u32), cs);
-      out_pieces = (Point*)dev_alloc(2 * T * sizeof(Point), cs);
-      to_free.push_back(out_keys);
-      to_free.push_back(out_pieces);
-    }
-    const u32 fin = final_level ? 1u : 0u;
-    if (first) {
-      const u32 unit_z = (walk_gens == gens && opt.gens_normalized) ? 1u : 0u;
-      // faster on ed25519 (a run start is a multiplication by a constant there); the Weierstrass
-      // start is free, so the extra addition loses
-      const bool uniform =
-          opt.uniform_add == 2 ? C::kCurveId == kRistretto255 : opt.uniform_add != 0;
-      if (uniform)
-        launch(AccumulateBody<C, true, SeqExec, true>{nullptr, walk_entries, walk_gens, nullptr,
-                                                      m_ptr, K, fin, d_target, out_keys, out_pieces,
-                                                      out_m, unit_z},
-               T, s);
-      else
-        launch(AccumulateBody<C, true>{nullptr, walk_entries, walk_gens, nullptr, m_ptr, K, fin,
-                                       d_target, out_keys, out_pieces, out_m, unit_z},
-               T, s);
-      KernelTimer::get().end(s);
-      if (tail != s) {
-        stream_follow(tail, s);
-        cs = tail;
-      }
-    } else if (T <= opt.quad_threshold) {
-      launch(AccumulateBody<C, false, QuadExec>{lvl_keys, nullptr, nullptr, lvl_pieces, m_ptr, K,
-                                                fin, d_target, out_keys, out_pieces, out_m, 0u},
-             T * QuadExec::kLanes, cs);
-    } else {
-      launch(AccumulateBody<C, false>{lvl_keys, nullptr, nullptr, lvl_pieces, m_ptr, K, fin,
-                                      d_target, out_keys, out_pieces, out_m, 0u},
-             T, cs);
-    }
-    if (final_level)
-      break;
-    first = false;
-    lvl_keys = out_keys;
-    lvl_pieces = out_pieces;
-    m_ptr = out_m;
-    m_max = 2 * T;
-    K = chunkn;
-    ++level;
-  }
+  typedef typename C::Point Point;  // later ranges: own bucket array, merged into the shared one below
+  Point* target = add_into ? (Point*)dev_alloc(nkeys * sizeof(Point), s) : d_buckets;
+  const u32 unit_z = (walk.gens == gens && opt.gens_normalized) ? 1u : 0u;
+  const stream_t cs = chunk_walk<C>(s, tail, walk, sorted.d_m, unit_z, target, opt, to_free);
+  // What the later levels and the merge read on cs (pieces, keys, d_m, counts, starts) is freed on cs:
+  // freed on s, it could go to the next range's allocations while cs still reads it. So are the last
+  // pair level's points and entries. The sorted entries and the staged columns are read on s only.
   if (add_into) {
-    launch(MergeBucketsBody<C>{d_counts, d_starts, d_target, d_buckets}, nkeys, cs);
-    dev_free(d_target, cs);
+    launch(MergeBucketsBody<C>{sorted.counts, sorted.starts, target, d_buckets}, nkeys, cs);
+    dev_free(target, cs);
   }
+  to_free.insert(to_free.end(), {sorted.d_m, sorted.counts, sorted.starts});
   for (void* ptr : to_free)
     dev_free(ptr, cs);
-  dev_free(d_entries, s);
-  dev_free(d_m, cs);
-  dev_free(d_counts, cs);
-  dev_free(d_starts, cs);
-  dev_free(d_stage, s);
+  dev_free(sorted.entries, s);
+  dev_free((void*)r.d_cols, s);
 }
 
 // Bucket reduction + window combination: out[j] for every column of the plan.
