@@ -42,6 +42,7 @@ B200_SYMBOLS = [
     "b200_fixed_msm_host_partials", "b200_multiexp_handle_new_device",
     "b200_selftest_lane_arithmetic", "b200_selftest_sort", "b200_partition_table_device",
     "b200_multiexp_handle_write_partition_table",
+    "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
 ]
 
 
@@ -141,6 +142,31 @@ def compute_pedersen_commitments(curve_id, columns, generators=None, offset_gene
               2: L.sxt_bn254_g1_uncompressed_compute_pedersen_commitments_with_generators,
               3: L.sxt_grumpkin_uncompressed_compute_pedersen_commitments_with_generators}[curve_id]
         fn(_ptr(out), num, desc, _ptr(generators))
+    return out
+
+
+def _offsets(offsets, num):
+    if offsets is None:
+        return None
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    if offsets.shape != (num,):
+        raise ValueError(f"offsets must hold one entry per column ({num})")
+    return offsets
+
+
+def compute_pedersen_commitments_with_offsets(curve_id, columns, offsets, generators=None):
+    """b200_compute_pedersen_commitments_with_offsets: column j pairs row i with generator
+    offsets[j] + i, all columns in one engine pass (offsets None = all 0).
+
+    generators: uint8 array [m, stride] in the ABI layout of the curve, indexed by offsets[j] + i
+    (None = built-in ristretto generators). Returns uint8 [num_columns, commitment bytes].
+    """
+    desc, keep = make_descriptors(columns)
+    offsets = _offsets(offsets, len(columns))
+    out = np.zeros((len(columns), CURVE_SIZES[curve_id][2]), dtype=np.uint8)
+    lib().b200_compute_pedersen_commitments_with_offsets(
+        C.c_uint(curve_id), _ptr(out), C.c_uint32(len(columns)), desc, _ptr(generators),
+        _ptr(offsets))
     return out
 
 
@@ -272,6 +298,23 @@ def commit_device(curve_id, columns_shape, scalar_ptrs, generators_ptr, out_comm
     lib().b200_commit_device(C.c_uint(curve_id), C.c_void_p(out_commit_ptr),
                              C.c_void_p(out_partial_ptr), C.c_uint32(num), arr,
                              C.c_void_p(generators_ptr), C.c_uint64(offset_generators))
+
+
+def commit_device_with_offsets(curve_id, columns_shape, scalar_ptrs, generators_ptr, offsets,
+                               out_commit_ptr=None, out_partial_ptr=None):
+    """b200_commit_device_with_offsets: as commit_device, column j at generator offsets[j] (a host
+    array; None = all 0)."""
+    num = len(columns_shape)
+    arr = (sxt_sequence_descriptor * max(1, num))()
+    for i, (n, nbytes, is_signed) in enumerate(columns_shape):
+        arr[i].element_nbytes = nbytes
+        arr[i].n = n
+        arr[i].data = scalar_ptrs[i]
+        arr[i].is_signed = int(is_signed)
+    offsets = _offsets(offsets, num)
+    lib().b200_commit_device_with_offsets(C.c_uint(curve_id), C.c_void_p(out_commit_ptr),
+                                          C.c_void_p(out_partial_ptr), C.c_uint32(num), arr,
+                                          C.c_void_p(generators_ptr), _ptr(offsets))
 
 
 def selftest_lane_arithmetic(warps=64, seed=1):

@@ -338,10 +338,12 @@ void wait_for_range(void* user, uint64_t begin, uint64_t end) {
 
 // the commitments of `num` columns on one device (the calling thread's current device is st.device)
 // Results: `commitments` (host, canonical) or, when out_partials_dev is given instead, the internal
-// accumulator points in device memory (multi-GPU callers combine them).
+// accumulator points in device memory (multi-GPU callers combine them). offsets (host, optional):
+// column j starts at generator offsets[j]; offset_generators is then unused.
 void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t num,
                const sxt_sequence_descriptor* d, const void* generators,
-               uint64_t offset_generators, void* out_partials_dev = nullptr) {
+               uint64_t offset_generators, void* out_partials_dev = nullptr,
+               const uint64_t* offsets = nullptr) {
   const CurveVTable& V = vt(curve_id);
   StageRange nvtx("commit (host buffers)");
   cudaStream_t s = st.stream, sc = st.copy_stream;
@@ -349,7 +351,9 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
   size_t total_scalar_bytes = 0;
   for (uint32_t i = 0; i < num; ++i)
     total_scalar_bytes += (size_t)d[i].n * d[i].element_nbytes + 32;
-  DevBuf<unsigned char> raw_gens(generators ? n * V.abi_gen_bytes : 1, s);
+  // per-column offsets: the device holds only the generators the columns use, in the packed order
+  std::unique_ptr<GenLayout> layout(offsets ? new GenLayout(d, num, offsets) : nullptr);
+  DevBuf<unsigned char> raw_gens(generators ? (layout ? layout->total : n) * V.abi_gen_bytes : 1, s);
   DevBuf<unsigned char> scal(total_scalar_bytes, s);
   DevBuf<unsigned char> out((size_t)num * V.abi_commit_bytes, s);
   std::vector<sxt_sequence_descriptor> dd(d, d + num);
@@ -405,10 +409,16 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
                              d[i].data + lo * d[i].element_nbytes,
                              (hi - lo) * d[i].element_nbytes, sc);
     }
-    if (generators)
+    if (generators && layout) {
+      for (const GenLayout::Piece& p : layout->needed(b, e))
+        HostStager::get().copy(raw_gens.p + p.pos * V.abi_gen_bytes,
+                               static_cast<const unsigned char*>(generators) + p.src * V.abi_gen_bytes,
+                               p.count * V.abi_gen_bytes, sc);
+    } else if (generators) {
       HostStager::get().copy(raw_gens.p + b * V.abi_gen_bytes,
                              static_cast<const unsigned char*>(generators) + b * V.abi_gen_bytes,
                              (e - b) * V.abi_gen_bytes, sc);
+    }
     B200_CUDA(cudaEventRecord(st.range_events[r], sc));
     mark(sc);
   };
@@ -418,9 +428,14 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
   RangeWaitState w{n, num_ranges, skew, &st, 0, upload};
   EngineCtx cx = ctx_of(st);
   cx.opt.range_skew = skew;
-  V.commit_device(cx, out_partials_dev ? nullptr : out.p, out_partials_dev, num, dd.data(),
-                  generators ? raw_gens.p : nullptr, offset_generators, num_ranges, &wait_for_range,
-                  &w);
+  if (layout)
+    V.commit_device_offsets(cx, out_partials_dev ? nullptr : out.p, out_partials_dev, num, dd.data(),
+                            generators ? raw_gens.p : nullptr, offsets, true, num_ranges,
+                            &wait_for_range, &w);
+  else
+    V.commit_device(cx, out_partials_dev ? nullptr : out.p, out_partials_dev, num, dd.data(),
+                    generators ? raw_gens.p : nullptr, offset_generators, num_ranges, &wait_for_range,
+                    &w);
   mark(s);
   if (!out_partials_dev)
     copy_d2h(commitments, out.p, (size_t)num * V.abi_commit_bytes, s);
@@ -556,7 +571,8 @@ void send_partials(const State& st, size_t part, const void* partials_dev, size_
 
 void commit_host(unsigned curve_id, void* commitments, uint32_t num,
                  const sxt_sequence_descriptor* d, const void* generators,
-                 uint64_t offset_generators, const char* fn, void* out_partials_dev = nullptr) {
+                 uint64_t offset_generators, const char* fn, void* out_partials_dev = nullptr,
+                 const uint64_t* offsets = nullptr) {
   if (num == 0)
     return;
   std::lock_guard<std::mutex> lock(g_mutex);
@@ -565,12 +581,14 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
   const uint64_t n = longest_column(d, num);  // validates the descriptors before any thread starts
   if (curve_id != SXT_CURVE_RISTRETTO255)
     B200_REQUIRE(generators != nullptr, "generators == nullptr");
+  if (offsets)
+    (void)GenLayout(d, num, offsets);  // validates the offsets before any thread starts
   const CurveVTable& V = vt(curve_id);
   const size_t stride = V.abi_commit_bytes;
   const size_t devices = g_workers.size() + 1;
   if (devices <= 1 || out_partials_dev) {
     commit_on(g_state, curve_id, commitments, num, d, generators, offset_generators,
-              out_partials_dev);
+              out_partials_dev, offsets);
     return;
   }
   if (num >= devices) {
@@ -589,7 +607,8 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
     }
     on_devices(parts, [&, curve_id, commitments, d, generators, offset_generators](size_t p) {
       commit_on(state_of(p), curve_id, static_cast<unsigned char*>(commitments) + cut[p] * stride,
-                cut[p + 1] - cut[p], d + cut[p], generators, offset_generators);
+                cut[p + 1] - cut[p], d + cut[p], generators, offset_generators, nullptr,
+                offsets ? offsets + cut[p] : nullptr);
     });
     return;
   }
@@ -598,7 +617,8 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
   // the primary device and summed there (the MSM is linear)
   const size_t parts = range_parts(n);
   if (parts <= 1) {
-    commit_on(g_state, curve_id, commitments, num, d, generators, offset_generators);
+    commit_on(g_state, curve_id, commitments, num, d, generators, offset_generators, nullptr,
+              offsets);
     return;
   }
   const size_t pbytes = (size_t)num * V.point_bytes;
@@ -608,15 +628,22 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
     State& st = state_of(p);
     const uint64_t lo = n * p / parts, hi = n * (p + 1) / parts;
     std::vector<sxt_sequence_descriptor> dd(d, d + num);
-    for (auto& c : dd) {
+    std::vector<uint64_t> part_offsets(offsets ? num : 0);  // each column's slice starts at row b
+    for (uint32_t j = 0; j < num; ++j) {
+      auto& c = dd[j];
       const uint64_t b = std::min<uint64_t>(lo, c.n), e = std::min<uint64_t>(hi, c.n);
       c.data = c.data ? c.data + b * c.element_nbytes : nullptr;
       c.n = e - b;
+      if (offsets)
+        part_offsets[j] = offsets[j] + b;
     }
     const unsigned char* g = static_cast<const unsigned char*>(generators);
     DevBuf<unsigned char> part(pbytes, st.stream);
-    commit_on(st, curve_id, nullptr, num, dd.data(), g ? g + lo * V.abi_gen_bytes : nullptr,
-              offset_generators + lo, part.p);
+    if (offsets)
+      commit_on(st, curve_id, nullptr, num, dd.data(), g, 0, part.p, part_offsets.data());
+    else
+      commit_on(st, curve_id, nullptr, num, dd.data(), g ? g + lo * V.abi_gen_bytes : nullptr,
+                offset_generators + lo, part.p);
     send_partials(st, p, part.p, pbytes, gather);
   });
   cudaStream_t s = g_state.stream;
@@ -1182,6 +1209,29 @@ void b200_commit_device(unsigned curve_id, void* out_commitments, void* out_part
   require_init("b200_commit_device");
   vt(curve_id).commit_device(ctx(), out_commitments, out_partials, num_sequences, descriptors,
                              generators, offset_generators, 1, nullptr, nullptr);
+}
+void b200_compute_pedersen_commitments_with_offsets(unsigned curve_id, void* commitments,
+                                                    uint32_t num_sequences,
+                                                    const struct sxt_sequence_descriptor* descriptors,
+                                                    const void* generators, const uint64_t* offsets) {
+  commit_host(curve_id, commitments, num_sequences, descriptors, generators, 0,
+              "b200_compute_pedersen_commitments_with_offsets", nullptr, offsets);
+}
+void b200_commit_device_with_offsets(unsigned curve_id, void* out_commitments, void* out_partials,
+                                     uint32_t num_sequences,
+                                     const struct sxt_sequence_descriptor* descriptors,
+                                     const void* generators, const uint64_t* offsets) {
+  if (num_sequences == 0)
+    return;
+  std::lock_guard<std::mutex> lock(g_mutex);
+  require_init("b200_commit_device_with_offsets");
+  const CurveVTable& V = vt(curve_id);
+  if (offsets)
+    V.commit_device_offsets(ctx(), out_commitments, out_partials, num_sequences, descriptors,
+                            generators, offsets, false, 1, nullptr, nullptr);
+  else
+    V.commit_device(ctx(), out_commitments, out_partials, num_sequences, descriptors, generators,
+                    0, 1, nullptr, nullptr);
 }
 void b200_commit_host_partials(unsigned curve_id, void* out_partials,
                                uint32_t num_sequences,

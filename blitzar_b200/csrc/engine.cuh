@@ -108,6 +108,99 @@ template <class C> struct CurveOps {
       die("generators == nullptr", __FILE__, __LINE__);
   }
 
+  // generator ingestion / generation of one range with per-column generator starts: every piece of
+  // GenLayout::needed in one launch
+  struct PiecesHook : RangeHook {
+    const EngineCtx* ctx;
+    const GenLayout* layout;
+    const unsigned char* raw;  // ABI-layout generators on the device, or null
+    bool packed;               // raw is in the layout's packed order (else indexed by source index)
+    bool generate;             // generate built-in generators instead of converting `raw`
+    Gen* gens;                 // the packed device generators
+    range_wait_fn wait;
+    void* wait_user;
+    bool pending = false;  // an ingestion is running on the second stream
+    void before_range(u64 begin, u64 end) override {
+      end = std::min<u64>(end, layout->max_n);
+      if (begin >= end)
+        return;
+      if (wait)
+        wait(wait_user, begin, end);
+      if (!raw && !generate)
+        return;
+      const std::vector<GenLayout::Piece> pieces = layout->needed(begin, end);
+      const size_t np = pieces.size();
+      std::vector<u64> block(3 * np + 1, 0);  // [start x (np + 1)][from x np][to x np]
+      for (size_t k = 0; k < np; ++k) {
+        block[k + 1] = block[k] + pieces[k].count;
+        block[np + 1 + k] = raw && packed ? pieces[k].pos : pieces[k].src;
+        block[2 * np + 1 + k] = pieces[k].pos;
+      }
+      // as in IngestHook: the ingestion runs under the range's sort on a second stream
+      const stream_t on = raw ? aux_stream() : ctx->s;
+      if (raw)
+        stream_follow(on, ctx->s);
+      const u64* staged = (const u64*)stage_to_device(on, block.data(), block.size() * sizeof(u64));
+      const GenPieces p{staged, staged + np + 1, staged + 2 * np + 1, (u32)np};
+      if (raw) {
+        launch(IngestPiecesBody<C>{raw, gens, p}, block[np], on);
+        pending = true;
+      } else if constexpr (C::kCurveId == kRistretto255) {
+        launch(BuiltinPiecesBody{gens, p}, block[np], on);
+      }
+      dev_free((void*)staged, on);
+    }
+    void before_accumulate() override {
+      if (pending) {
+        stream_follow(ctx->s, aux_stream());
+        pending = false;
+      }
+    }
+  };
+
+  static std::vector<ColumnDesc> columns_of(const sxt_sequence_descriptor* d, uint32_t num) {
+    std::vector<ColumnDesc> cols(num);
+    for (uint32_t i = 0; i < num; ++i) {
+      cols[i].base = d[i].data;
+      cols[i].row_stride = d[i].element_nbytes;
+      cols[i].bit_offset = 0;
+      cols[i].bit_width = 8u * d[i].element_nbytes;
+      cols[i].n = (u32)d[i].n;
+      cols[i].is_signed = d[i].is_signed ? 1u : 0u;
+      cols[i].first_window = cols[i].num_windows = 0;
+      cols[i].table_n = 0;
+    }
+    return cols;
+  }
+
+  // the commitments (or partial points) of `cols` over `gens`; builtin_table: gens is the built-in
+  // generator array, whose fixed-base table serves the call when it is the cheaper run
+  static void commit_columns(const EngineCtx& ctx, void* out_commitments, void* out_partials,
+                             std::vector<ColumnDesc>& cols, const Gen* gens, bool builtin_table,
+                             uint32_t num_ranges, RangeHook* hook) {
+    stream_t s = ctx.s;
+    const uint32_t num = (uint32_t)cols.size();
+    Point* pts = (Point*)out_partials;
+    DevBuf<Point> tmp(out_partials ? 1 : num, s);
+    if (!pts)
+      pts = tmp.p;
+    EngineCtx rctx = ctx;
+    if (builtin_table && ctx.builtin_windows > 1)
+      rctx.opt.gens_normalized = 1u;  // the built-in table's entries are normalised (Z = 1)
+    // built-in generators covered by the precomputed fixed-base table (sxt_config::
+    // num_precomputed_generators): shared-bucket table mode when it is the cheaper run
+    if (builtin_table &&
+        prefer_table(cols, ctx.builtin_window_bits, ctx.builtin_windows, ctx.opt)) {
+      rctx.opt.window_bits = ctx.builtin_window_bits;
+      for (auto& col : cols)
+        col.table_n = (u32)ctx.num_builtin;
+    }
+    run_columns(rctx, gens, cols, pts, num_ranges ? num_ranges : 1, hook);
+    hook->before_accumulate();  // (no-op unless a range was ingested without being accumulated)
+    if (out_commitments)
+      launch_store_commit<C>(s, pts, (unsigned char*)out_commitments, num, ctx.opt.lane_tail != 0);
+  }
+
   // device-resident variable-base MSM; descriptors[i].data and generators_dev are device pointers.
   // The generator range is processed in num_ranges pieces; `wait` (optional) is called on the host
   // before each piece is touched.
@@ -136,36 +229,40 @@ template <class C> struct CurveOps {
       else
         hook.builtin = true;
     }
-    std::vector<ColumnDesc> cols(num);
-    for (uint32_t i = 0; i < num; ++i) {
-      cols[i].base = d[i].data;
-      cols[i].row_stride = d[i].element_nbytes;
-      cols[i].bit_offset = 0;
-      cols[i].bit_width = 8u * d[i].element_nbytes;
-      cols[i].n = (u32)d[i].n;
-      cols[i].is_signed = d[i].is_signed ? 1u : 0u;
-      cols[i].first_window = cols[i].num_windows = 0;
-      cols[i].table_n = 0;
-    }
-    Point* pts = (Point*)out_partials;
-    DevBuf<Point> tmp(out_partials ? 1 : num, s);
-    if (!pts)
-      pts = tmp.p;
-    EngineCtx rctx = ctx;
-    if (n && !generators_dev && !hook.builtin && ctx.builtin_windows > 1)
-      rctx.opt.gens_normalized = 1u;  // the built-in table's entries are normalised (Z = 1)
-    // built-in generators covered by the precomputed fixed-base table (sxt_config::
-    // num_precomputed_generators): shared-bucket table mode when it is the cheaper run
-    if (n && !generators_dev && !hook.builtin &&
-        prefer_table(cols, ctx.builtin_window_bits, ctx.builtin_windows, ctx.opt)) {
-      rctx.opt.window_bits = ctx.builtin_window_bits;
-      for (auto& col : cols)
-        col.table_n = (u32)ctx.num_builtin;
-    }
-    run_columns(rctx, gens_ptr, cols, pts, num_ranges ? num_ranges : 1, &hook);
-    hook.before_accumulate();  // (no-op unless a range was ingested without being accumulated)
-    if (out_commitments)
-      launch_store_commit<C>(s, pts, (unsigned char*)out_commitments, num, ctx.opt.lane_tail != 0);
+    std::vector<ColumnDesc> cols = columns_of(d, num);
+    commit_columns(ctx, out_commitments, out_partials, cols, gens_ptr,
+                   n && !generators_dev && !hook.builtin, num_ranges, &hook);
+  }
+
+  // commit_device with a generator start per column: row i of column j pairs with generator
+  // offsets[j] + i (offsets null = all 0). The generators the columns use are laid out by GenLayout;
+  // only built-in generators that all lie in the precomputed range are used in place.
+  static void commit_device_offsets(const EngineCtx& ctx, void* out_commitments,
+                                    void* out_partials, uint32_t num,
+                                    const sxt_sequence_descriptor* d, const void* generators_dev,
+                                    const uint64_t* offsets, bool packed, uint32_t num_ranges,
+                                    range_wait_fn wait, void* wait_user) {
+    check_descriptors(d, num);
+    const GenLayout layout(d, num, offsets);
+    if (layout.total && !generators_dev && C::kCurveId != kRistretto255)
+      die("generators == nullptr", __FILE__, __LINE__);
+    const bool builtin_table = layout.total && !generators_dev && layout.within(ctx.num_builtin);
+    DevBuf<Gen> gens(builtin_table ? 1 : layout.total, ctx.s);
+    PiecesHook hook;
+    hook.ctx = &ctx;
+    hook.layout = &layout;
+    hook.raw = (const unsigned char*)generators_dev;
+    hook.packed = packed;
+    hook.generate = layout.total && !generators_dev && !builtin_table;
+    hook.gens = gens.p;
+    hook.wait = wait;
+    hook.wait_user = wait_user;
+    std::vector<ColumnDesc> cols = columns_of(d, num);
+    for (uint32_t j = 0; j < num; ++j)  // built-in array: generator g sits at position g
+      cols[j].gen_base = builtin_table && d[j].n && offsets ? (u32)offsets[j] : layout.base[j];
+    commit_columns(ctx, out_commitments, out_partials, cols,
+                   builtin_table ? (const Gen*)ctx.builtin : gens.p, builtin_table, num_ranges,
+                   &hook);
   }
 
   // fixed-base MSM over a handle's device-resident generators (mode 0 fixed width, 1 packed, 2 vlen)
@@ -301,6 +398,7 @@ template <class C> struct CurveOps {
                             (unsigned)C::kAbiProjBytes,                                            \
                             (unsigned)C::kAbiCommitBytes,                                          \
                             &CurveOps<C>::commit_device,                                           \
+                            &CurveOps<C>::commit_device_offsets,                                   \
                             &CurveOps<C>::fixed_device,                                            \
                             &CurveOps<C>::ingest_projective,                                       \
                             &CurveOps<C>::gens_to_projective,                                      \

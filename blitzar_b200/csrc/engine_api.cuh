@@ -1,8 +1,10 @@
 // Type-erased per-curve entry points of the MSM engine. api.cu sees only this header, so the
 // kernels of each curve are compiled exactly once, in that curve's own translation unit.
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <vector>
 
 #include "../../include/blitzar_b200.h"
 #include "runtime.cuh"
@@ -106,12 +108,93 @@ inline uint64_t range_begin(uint64_t n, uint32_t r, uint32_t num_ranges, int ske
 // for that range's copies)
 typedef void (*range_wait_fn)(void* user, uint64_t begin, uint64_t end);
 
+// Generator layout of a call whose column j pairs row i with generator offsets[j] + i (offsets null =
+// all 0). The intervals [offsets[j], offsets[j] + n_j) of the non-empty columns, merged where they
+// overlap or touch, are packed in increasing order into one array; column j's generator of row i
+// sits at packed position base[j] + i. The engine (ingestion / generation per range) and the C-ABI
+// layer (raw buffer size, upload pieces) both take the layout from here.
+struct GenLayout {
+  struct Piece {
+    uint64_t src, pos, count;  // generators [src, src + count) of the source at packed [pos, pos + count)
+  };
+  std::vector<Piece> segments;  // the merged intervals
+  std::vector<uint32_t> base;   // per column (0 for an empty column)
+  uint64_t total = 0;           // packed size
+  uint64_t max_n = 0;           // longest column
+
+  GenLayout(const sxt_sequence_descriptor* d, uint32_t num, const uint64_t* offsets)
+      : base(num, 0), n_(num, 0) {
+    std::vector<uint32_t> order;
+    for (uint32_t j = 0; j < num; ++j) {
+      n_[j] = d[j].n;
+      max_n = std::max<uint64_t>(max_n, d[j].n);
+      if (d[j].n) {
+        B200_REQUIRE(offset(offsets, j) <= ~0ull - d[j].n, "generator offset + column length overflows");
+        order.push_back(j);
+      }
+    }
+    std::stable_sort(order.begin(), order.end(), [offsets](uint32_t a, uint32_t b) {
+      return offset(offsets, a) < offset(offsets, b);
+    });
+    for (uint32_t j : order) {
+      const uint64_t lo = offset(offsets, j), hi = lo + n_[j];
+      if (segments.empty() || lo > segments.back().src + segments.back().count) {
+        const uint64_t pos = segments.empty() ? 0 : segments.back().pos + segments.back().count;
+        segments.push_back({lo, pos, 0});
+      }
+      Piece& s = segments.back();
+      s.count = std::max(s.count, hi - s.src);
+      B200_REQUIRE(s.pos + s.count < (1ull << 31),
+                   "merged generator intervals of 2^31 or more generators");
+      base[j] = (uint32_t)(s.pos + (lo - s.src));
+    }
+    total = segments.empty() ? 0 : segments.back().pos + segments.back().count;
+  }
+  // every interval ends at or below `limit`
+  bool within(uint64_t limit) const {
+    return segments.empty() || segments.back().src + segments.back().count <= limit;
+  }
+  // the generators rows [b, e) of the columns use: U_j [base_j + b, base_j + min(e, n_j)), merged
+  // within each segment, in increasing packed order
+  std::vector<Piece> needed(uint64_t b, uint64_t e) const {
+    std::vector<std::pair<uint64_t, uint64_t>> iv;  // packed [lo, hi)
+    for (size_t j = 0; j < base.size(); ++j)
+      if (n_[j] > b)
+        iv.push_back({base[j] + b, base[j] + std::min(e, n_[j])});
+    std::sort(iv.begin(), iv.end());
+    std::vector<Piece> out;
+    size_t k = 0;  // segment of the current interval (intervals never cross a segment)
+    for (auto& v : iv) {
+      while (segments[k].pos + segments[k].count <= v.first)
+        ++k;
+      const Piece& s = segments[k];
+      if (!out.empty() && out.back().pos + out.back().count >= v.first && out.back().pos >= s.pos) {
+        out.back().count = std::max(out.back().count, v.second - out.back().pos);
+        continue;
+      }
+      out.push_back({s.src + (v.first - s.pos), v.first, v.second - v.first});
+    }
+    return out;
+  }
+
+private:
+  std::vector<uint64_t> n_;
+  static uint64_t offset(const uint64_t* offsets, uint32_t j) { return offsets ? offsets[j] : 0; }
+};
+
 struct CurveVTable {
   unsigned curve_id, point_bytes, gen_bytes, abi_gen_bytes, abi_proj_bytes, abi_commit_bytes;
   void (*commit_device)(const EngineCtx&, void* out_commitments, void* out_partials, uint32_t num,
                         const sxt_sequence_descriptor* d, const void* generators_dev,
                         uint64_t offset_generators, uint32_t num_ranges, range_wait_fn wait,
                         void* wait_user);
+  // as commit_device with generator offsets[j] + i for row i of column j (offsets: host array, null
+  // = all 0). generators_dev is indexed by offsets[j] + i, or, with `packed`, already holds
+  // GenLayout's packed array (host calls upload only the generators the columns use)
+  void (*commit_device_offsets)(const EngineCtx&, void* out_commitments, void* out_partials,
+                                uint32_t num, const sxt_sequence_descriptor* d,
+                                const void* generators_dev, const uint64_t* offsets, bool packed,
+                                uint32_t num_ranges, range_wait_fn wait, void* wait_user);
   void (*fixed_device)(const EngineCtx&, void* out_res, void* out_partials, const Handle* h,
                        int mode, unsigned element_num_bytes, const unsigned* bit_table,
                        const unsigned* lengths, unsigned num_outputs, unsigned n,

@@ -51,7 +51,9 @@ struct ColumnDesc {
   // column share ONE bucket set (first_window), so there is no Horner tail. 0 = one bucket set per
   // window (variable-base).
   u32 table_n;
-  u32 reserved_;
+  // generator of row i (window w) is gens[gen_base + i + w * table_n], gens being the generator
+  // pointer of the current range: per-column generator starts (commit_device_offsets); 0 otherwise
+  u32 gen_base;
 };
 B200_HD u32 bucket_windows(const ColumnDesc& col) { return col.table_n ? (col.num_windows ? 1u : 0u) : col.num_windows; }
 
@@ -229,7 +231,7 @@ struct ScatterBody {
     load_scalar_bits(v, neg, col, i);
     u32* cur = cursor;
     u64* en = entries;
-    const u32 ii = (u32)i, tn = col.table_n;
+    const u32 ii = (u32)i + col.gen_base, tn = col.table_n;
     for_each_digit(v, neg, col, c, nbuckets, [cur, en, ii, tn](u32 key, bool negate, u32 w) {
       u32 pos = B200_ATOMIC_ADD(&cur[key], 1u);
       en[pos] = ((u64)key << 32) | (u64)(((ii + w * tn) << 1) | (negate ? 1u : 0u));
@@ -359,7 +361,7 @@ __device__ void for_each_entry(const ColumnDesc* cols, const u64* col_start, u32
   u32 v[8];
   bool neg;
   load_scalar_bits(v, neg, col, i);
-  const u32 ii = (u32)i, tn = col.table_n;
+  const u32 ii = (u32)i + col.gen_base, tn = col.table_n;
   for_each_digit(v, neg, col, c, nbuckets, [&](u32 key, bool negate, u32 w) {
     f(key, ((u64)key << 32) | (u64)(((ii + w * tn) << 1) | (negate ? 1u : 0u)));
   });
@@ -1061,6 +1063,34 @@ struct BuiltinGeneratorBody {
     Ed25519::point_to_gen(gens[i], g);
   }
 };
+// Several pieces of generators in one launch (per-column generator starts, GenLayout): piece k moves
+// start[k+1] - start[k] generators from source index from[k] to device position to[k]. A thread finds
+// its piece by binary search over the prefix `start`, then runs the one-piece body's element code.
+struct GenPieces {
+  const u64* start;  // [npieces + 1]
+  const u64* from;   // [npieces]
+  const u64* to;     // [npieces]
+  u32 npieces;
+};
+template <class C> struct IngestPiecesBody {
+  static constexpr int kBlock = IngestBody<C, false>::kBlock;
+  const unsigned char* raw;  // ABI-layout generators, indexed by `from`
+  typename C::Gen* gens;
+  GenPieces p;
+  B200_HD void operator()(u64 tid) const {
+    const u32 k = column_of(p.start, p.npieces, tid);
+    IngestBody<C, false>{raw + p.from[k] * C::kAbiGenBytes, gens + p.to[k]}(tid - p.start[k]);
+  }
+};
+struct BuiltinPiecesBody {
+  static constexpr int kBlock = BuiltinGeneratorBody::kBlock;
+  Ed25519::Gen* gens;
+  GenPieces p;  // `from` = index of the built-in generator
+  B200_HD void operator()(u64 tid) const {
+    const u32 k = column_of(p.start, p.npieces, tid);
+    BuiltinGeneratorBody{gens + p.to[k], p.from[k]}(tid - p.start[k]);
+  }
+};
 // result canonicalisation
 template <class C, bool kCommit> struct StoreBody {
   static constexpr int kBlock = 32;
@@ -1161,6 +1191,10 @@ inline MsmPlan msm_make_plan(std::vector<ColumnDesc> cols, const MsmOptions& opt
     max_entries += (u64)col.n * col.num_windows;
     if (col.table_n)
       B200_REQUIRE((u64)col.table_n * col.num_windows < (1ull << 31), "generator table too large");
+    // the largest generator index of the column's entries fits the entry's 31-bit field
+    if (col.n)
+      B200_REQUIRE((u64)col.gen_base + col.n + (u64)(col.num_windows - 1) * col.table_n < (1ull << 31),
+                   "generator index of a column too large");
   }
   p.nkeys = (u64)p.total_windows * p.nbuckets;
   p.total_entries = max_entries;

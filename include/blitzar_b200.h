@@ -191,6 +191,20 @@ void b200_commit_device(unsigned curve_id, void* out_commitments, void* out_part
 void b200_commit_host_partials(unsigned curve_id, void* out_partials, uint32_t num_sequences,
                                const struct sxt_sequence_descriptor* descriptors,
                                const void* generators, uint64_t offset_generators);
+/* commitments[j] = sum_i a_ij * g(offsets[j] + i), all columns in one engine pass. generators ==
+ * NULL: built-in ristretto generators (curve 0 only); else the caller's array in the layout / stride
+ * of the curve's sxt_*_with_generators call. offsets == NULL: all 0. commitments in the layout of
+ * the matching sxt_* call. Host pointers; synchronises. */
+void b200_compute_pedersen_commitments_with_offsets(unsigned curve_id, void* commitments,
+                                                    uint32_t num_sequences,
+                                                    const struct sxt_sequence_descriptor* descriptors,
+                                                    const void* generators, const uint64_t* offsets);
+/* as b200_commit_device (device descriptors / generators, out_commitments and / or out_partials,
+ * no synchronisation); offsets is a HOST array */
+void b200_commit_device_with_offsets(unsigned curve_id, void* out_commitments, void* out_partials,
+                                     uint32_t num_sequences,
+                                     const struct sxt_sequence_descriptor* descriptors,
+                                     const void* generators, const uint64_t* offsets);
 /* as the three sxt_fixed_* calls (host scalars; mode 0 fixed width, 1 packed, 2 vlen), partial
  * accumulator points to device memory */
 void b200_fixed_msm_host_partials(void* out_partials, const struct sxt_multiexp_handle* handle,
