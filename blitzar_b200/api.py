@@ -43,6 +43,7 @@ B200_SYMBOLS = [
     "b200_selftest_lane_arithmetic", "b200_selftest_sort", "b200_partition_table_device",
     "b200_multiexp_handle_write_partition_table",
     "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
+    "b200_multiexp_handle_add_partition_table", "b200_multiexp_handle_partition_window",
 ]
 
 
@@ -213,6 +214,18 @@ class MultiexpHandle:
         sxt_multiexp_handle_new_from_file. window_width 0 = the reference's default."""
         lib().b200_multiexp_handle_write_partition_table(C.c_void_p(self.h), filename.encode(),
                                                          C.c_uint(window_width))
+
+    def add_partition_table(self, window_width=0):
+        """b200_multiexp_handle_add_partition_table: keeps the partition table of the given width
+        (0 = the reference's default) on the handle, so that narrow outputs are answered by table
+        lookups. Returns the width attached, or 0 when the table does not fit in HBM."""
+        return int(lib().b200_multiexp_handle_add_partition_table(C.c_void_p(self.h),
+                                                                  C.c_uint(window_width)))
+
+    @property
+    def partition_window(self):
+        """Width of the handle's partition table (0 = none)."""
+        return int(lib().b200_multiexp_handle_partition_window(C.c_void_p(self.h)))
 
     def free(self):
         if self.h:

@@ -74,6 +74,8 @@ EngineCtx ctx_of(const State& st) {
     c.opt.pair_batch = (u32)std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_TABLE_POLICY"))  // 1 = always use tables, 2 = never
     c.opt.table_policy = (u32)std::atoi(env);
+  if (const char* env = std::getenv("BLITZAR_B200_PARTITION_POLICY"))  // 1 = always, 2 = never
+    c.partition_policy = (u32)std::atoi(env);
   return c;
 }
 EngineCtx ctx() { return ctx_of(g_state); }
@@ -696,6 +698,82 @@ Handle* shard_new(const State& st, unsigned curve_id, const void* generators, un
   return h;
 }
 
+// Window width of the reference's partition tables: 1..24, the range sxt_multiexp_handle_new_from_
+// file reads; 0 = the reference's default, BLITZAR_PARTITION_WINDOW_WIDTH or else 16
+// (mtxpp2::get_default_window_width, sxt/multiexp/pippenger2/window_width.cc).
+unsigned partition_window(unsigned w) {
+  if (w == 0) {
+    const char* env = std::getenv("BLITZAR_PARTITION_WINDOW_WIDTH");
+    w = env ? (unsigned)std::strtoul(env, nullptr, 10) : 16u;
+  }
+  B200_REQUIRE(w >= 1 && w <= 24, "partition table window width must be in 1..24");
+  return w;
+}
+// Groups per chunk of a partition-table build: 64 MiB of compact entries (at least one group), or
+// what BLITZAR_B200_PTABLE_CHUNK_BYTES allows (test hook: many chunks). The build's scratch
+// (projective points, denominators, inversion tree) is up to 2.6x the chunk's entries.
+uint64_t partition_chunk_groups(const CurveVTable& V, unsigned w) {
+  uint64_t bytes = 64ull << 20;
+  if (const char* env = std::getenv("BLITZAR_B200_PTABLE_CHUNK_BYTES"))
+    bytes = std::strtoull(env, nullptr, 10);
+  return std::max<uint64_t>(1, bytes / ((uint64_t)V.abi_compact_bytes << w));
+}
+// Replaces shard h's partition table (Handle::ptable) with one of width w, built on st's device in
+// chunks of whole groups. The table may take at most 40 % of the free HBM, as the fixed-base tables
+// do (choose_table_window); false, and no table, when it does not fit.
+bool shard_add_partition_table(const State& st, Handle* h, unsigned w) {
+  const CurveVTable& V = vt(h->curve_id);
+  cudaStream_t s = st.stream;
+  stream_sync(s);
+  B200_CUDA(cudaFree(h->ptable));
+  h->ptable = nullptr;
+  h->ptable_w = 0;
+  h->ptable_groups = 0;
+  const uint64_t groups = ((uint64_t)h->n + w - 1) / w;
+  if (groups == 0)
+    return false;
+  size_t free_b = 0, total_b = 0;
+  B200_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const double bytes = std::ldexp((double)groups * V.gen_bytes, (int)w);
+  if (bytes > 0.4 * (double)free_b)
+    return false;
+  if (cudaMalloc(&h->ptable, (size_t)bytes) != cudaSuccess) {
+    cudaGetLastError();
+    h->ptable = nullptr;
+    return false;
+  }
+  const uint64_t step = partition_chunk_groups(V, w);
+  for (uint64_t g = 0; g < groups; g += step)
+    V.partition_gens(ctx_of(st), h->gens, h->n, w, g, std::min(step, groups - g),
+                     static_cast<unsigned char*>(h->ptable) + ((size_t)g << w) * V.gen_bytes);
+  stream_sync(s);
+  h->ptable_w = w;
+  h->ptable_groups = groups;
+  return true;
+}
+
+// every shard's partition table of width w (window_width 0 = the reference's default); the width, or
+// 0 (and no table on any shard) when a shard's table does not fit
+unsigned handle_add_partition_table(HandleSet* hs, unsigned window_width) {
+  const unsigned w = partition_window(window_width);
+  std::vector<char> ok(hs->shards.size(), 0);
+  on_devices(hs->shards.size(), [&, hs, w](size_t p) {
+    ok[p] = shard_add_partition_table(state_of(p), hs->shards[p], w) ? 1 : 0;
+  });
+  if (std::find(ok.begin(), ok.end(), 0) == ok.end())
+    return w;
+  on_devices(hs->shards.size(), [hs](size_t p) {
+    Handle* h = hs->shards[p];
+    stream_sync(state_of(p).stream);
+    B200_CUDA(cudaFree(h->ptable));
+    h->ptable = nullptr;
+    h->ptable_w = 0;
+    h->ptable_groups = 0;
+  });
+  B200_LOG(1, "partition table of width %u does not fit in 40 %% of the free HBM", w);
+  return 0;
+}
+
 HandleSet* handle_new(unsigned curve_id, const void* generators, unsigned n,
                       bool device_resident = false, unsigned compact_window = 0,
                       size_t compact_bytes = 0) {
@@ -724,6 +802,10 @@ HandleSet* handle_new(unsigned curve_id, const void* generators, unsigned n,
                               compact_window, cbytes);
   });
   (void)compact_bytes;
+  // lets an unmodified sxt_* consumer opt in to partition tables at the reference's default width
+  if (const char* env = std::getenv("BLITZAR_B200_PARTITION_HANDLES"))
+    if (std::atoi(env) == 1)
+      handle_add_partition_table(hs, 0);
   return hs;
 }
 
@@ -809,27 +891,6 @@ void fixed_host(void* res, const HandleSet* hs, int mode, unsigned element_num_b
 }
 
 const uint32_t kHandleMagic = 0x44483242u;  // "B2HD"
-
-// Window width of the reference's partition tables: 1..24, the range sxt_multiexp_handle_new_from_
-// file reads; 0 = the reference's default, BLITZAR_PARTITION_WINDOW_WIDTH or else 16
-// (mtxpp2::get_default_window_width, sxt/multiexp/pippenger2/window_width.cc).
-unsigned partition_window(unsigned w) {
-  if (w == 0) {
-    const char* env = std::getenv("BLITZAR_PARTITION_WINDOW_WIDTH");
-    w = env ? (unsigned)std::strtoul(env, nullptr, 10) : 16u;
-  }
-  B200_REQUIRE(w >= 1 && w <= 24, "partition table window width must be in 1..24");
-  return w;
-}
-// Groups per chunk of a partition-table build: 64 MiB of compact entries (at least one group), or
-// what BLITZAR_B200_PTABLE_CHUNK_BYTES allows (test hook: many chunks). The build's scratch
-// (projective points, denominators, inversion tree) is up to 2.6x the chunk's entries.
-uint64_t partition_chunk_groups(const CurveVTable& V, unsigned w) {
-  uint64_t bytes = 64ull << 20;
-  if (const char* env = std::getenv("BLITZAR_B200_PTABLE_CHUNK_BYTES"))
-    bytes = std::strtoull(env, nullptr, 10);
-  return std::max<uint64_t>(1, bytes / ((uint64_t)V.abi_compact_bytes << w));
-}
 
 }  // namespace
 
@@ -1032,6 +1093,7 @@ void sxt_multiexp_handle_free(struct sxt_multiexp_handle* handle) {
   on_devices(hs->shards.size(), [hs](size_t p) {
     B200_CUDA(cudaStreamSynchronize(state_of(p).stream));
     B200_CUDA(cudaFree(hs->shards[p]->gens));
+    B200_CUDA(cudaFree(hs->shards[p]->ptable));
     delete hs->shards[p];
   });
   delete hs;
@@ -1404,6 +1466,20 @@ void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle
     B200_CUDA(cudaEventDestroy(built[k]));
     B200_CUDA(cudaEventDestroy(copied[k]));
   }
+}
+unsigned b200_multiexp_handle_add_partition_table(struct sxt_multiexp_handle* handle,
+                                                  unsigned window_width) {
+  std::lock_guard<std::mutex> lock(g_mutex);
+  require_init("b200_multiexp_handle_add_partition_table");
+  HandleSet* hs = reinterpret_cast<HandleSet*>(handle);
+  B200_REQUIRE(hs != nullptr, "null handle");
+  return handle_add_partition_table(hs, window_width);
+}
+unsigned b200_multiexp_handle_partition_window(const struct sxt_multiexp_handle* handle) {
+  std::lock_guard<std::mutex> lock(g_mutex);
+  const HandleSet* hs = reinterpret_cast<const HandleSet*>(handle);
+  B200_REQUIRE(hs != nullptr, "null handle");
+  return hs->shards.empty() ? 0u : hs->shards[0]->ptable_w;
 }
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   std::lock_guard<std::mutex> lock(g_mutex);

@@ -8,6 +8,7 @@
 
 #include "engine_api.cuh"
 #include "msm.cuh"
+#include "partition_msm.cuh"
 #include "ptable.cuh"
 #include "synth.cuh"
 
@@ -302,6 +303,14 @@ template <class C> struct CurveOps {
     DevBuf<Point> tmp(out_partials ? 1 : (num_outputs ? num_outputs : 1), s);
     if (!pts)
       pts = tmp.p;
+    // outputs answered from the handle's partition table run as n = 0 columns of the engine
+    const std::vector<u32> routed = partition_route(ctx, h, cols);
+    std::vector<ColumnDesc> routed_cols;
+    if (!routed.empty()) {
+      routed_cols = cols;
+      for (u32 j : routed)
+        cols[j].n = 0;
+    }
     EngineCtx tctx = ctx;
     tctx.opt.gens_normalized = h->windows > 1 ? 1u : 0u;  // build_table normalised every entry
     if (prefer_table(cols, h->window_bits, h->windows, ctx.opt)) {
@@ -310,6 +319,7 @@ template <class C> struct CurveOps {
         col.table_n = h->n;
     }
     run_columns(tctx, (const Gen*)h->gens, cols, pts);
+    partition_msm<C>(s, (const Gen*)h->ptable, h->ptable_w, routed_cols, routed, pts);
     if (out_res)
       launch(StoreBody<C, false>{pts, (unsigned char*)out_res}, num_outputs, s);
   }
@@ -379,6 +389,49 @@ template <class C> struct CurveOps {
       }
     return cost_t < cost_v;
   }
+  // Outputs of a fixed-base call that the handle's partition table answers (DESIGN §4.4). Policy 0
+  // compares, per output of width b and length len, the table path's b ceil(len / w) lookups and b
+  // doublings with the engine's estimate as prefer_table makes it (table mode when the call would
+  // take it, else the variable-base run at the window width it would choose).
+  static std::vector<u32> partition_route(const EngineCtx& ctx, const Handle* h,
+                                          const std::vector<ColumnDesc>& cols) {
+    std::vector<u32> routed;
+    if (!h->ptable || ctx.partition_policy == 2)
+      return routed;
+    // cost of one table lookup / one bit of the Horner pass, in engine bucket-entry additions, fitted
+    // to the H100 timings of tests/partition_msm_timing.py (RESULTS §8): a lookup costs about what a
+    // bucket entry does, while the Horner pass is serial (b doublings and additions on one thread),
+    // so its latency weighs like 300 entries per bit
+    const double kLookup = 1.0, kDouble = 300.0;
+    const bool table_mode = prefer_table(cols, h->window_bits, h->windows, ctx.opt);
+    u64 max_n = 0;
+    u32 max_width = 1, ncols = 0;
+    for (auto& col : cols)
+      if (col.n) {
+        max_n = std::max<u64>(max_n, col.n);
+        max_width = std::max(max_width, col.bit_width);
+        ++ncols;
+      }
+    if (ncols == 0)
+      return routed;
+    const u32 cv = ctx.opt.window_bits ? ctx.opt.window_bits
+                                       : choose_window_bits(max_n, max_width, ncols, sizeof(Point));
+    const double nb_v = (double)(1u << (cv - 1)), w = h->ptable_w;
+    for (u32 j = 0; j < (u32)cols.size(); ++j) {
+      const ColumnDesc& col = cols[j];
+      if (col.n == 0)
+        continue;
+      const double n = col.n, b = col.bit_width;
+      const double engine =
+          table_mode ? n * (double)(col.bit_width / h->window_bits + 1) +
+                           2.5 * (double)(1u << (h->window_bits - 1))
+                     : (double)(col.bit_width / cv + 1) * (n + 2.5 * nb_v);
+      const double table = kLookup * b * std::ceil(n / w) + kDouble * b;
+      if (ctx.partition_policy == 1 || table < engine)
+        routed.push_back(j);
+    }
+    return routed;
+  }
   static void synth_generators(const EngineCtx& ctx, void* out_dev, uint64_t n, uint64_t first,
                                bool projective) {
     Synth<C>::generators(ctx.s, out_dev, n, first, projective);
@@ -387,6 +440,10 @@ template <class C> struct CurveOps {
                               uint64_t first_group, uint64_t groups, void* out_dev) {
     build_partition_table<C>(ctx.s, (const Gen*)gens, n, w, first_group, groups,
                              (unsigned char*)out_dev);
+  }
+  static void partition_gens(const EngineCtx& ctx, const void* gens, uint64_t n, unsigned w,
+                             uint64_t first_group, uint64_t groups, void* out_gens) {
+    build_partition_table<C>(ctx.s, (const Gen*)gens, n, w, first_group, groups, (Gen*)out_gens);
   }
 };
 
@@ -408,6 +465,7 @@ template <class C> struct CurveOps {
                             (unsigned)C::kAbiCompactBytes,                                         \
                             &CurveOps<C>::ingest_compact_table,                                    \
                             &CurveOps<C>::build_table,                                             \
-                            &CurveOps<C>::partition_table}
+                            &CurveOps<C>::partition_table,                                         \
+                            &CurveOps<C>::partition_gens}
 
 }  // namespace b200

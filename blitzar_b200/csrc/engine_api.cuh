@@ -44,16 +44,25 @@ struct EngineCtx {
   // fixed-base table over the built-in generators (window w of generator i at builtin[w n + i]);
   // builtin_windows <= 1: plain generators only
   u32 builtin_window_bits = 0, builtin_windows = 0;
+  // outputs of a fixed-base call over a handle with a partition table: 0 = cost model decides
+  // (partition_route), 1 = every non-empty output from the table, 2 = never from the table
+  u32 partition_policy = 0;
 };
 
 // sxt_multiexp_handle: generators of one curve resident in HBM, plus (when it pays and fits) the
 // fixed-base table 2^(c w) G_i, w < windows, laid out window-major: entry w * n + i. Window 0 IS the
 // generator array, so `gens` serves both the table mode and the variable-base fallback.
+// Optionally (b200_multiexp_handle_add_partition_table) also the reference's partition table of width
+// ptable_w over the same generators: 2^w subset sums per group of w generators, normalised device
+// generators at entry g * 2^w + k (partition_msm.cuh), the last group padded with the identity.
 struct Handle {
   unsigned curve_id;
   unsigned n;
   void* gens;  // device array of the curve's generator layout, windows * n entries
   unsigned window_bits = 0, windows = 1;
+  void* ptable = nullptr;  // partition table, ptable_groups << ptable_w entries (null = none)
+  unsigned ptable_w = 0;
+  uint64_t ptable_groups = 0;
 };
 
 // Window width of a fixed-base table over n generators: minimises (digit additions + bucket
@@ -218,6 +227,9 @@ struct CurveVTable {
   // generators (device generator layout; ptable.cuh) -> compact ABI entries at out_dev
   void (*partition_table)(const EngineCtx&, const void* gens, uint64_t n, unsigned w,
                           uint64_t first_group, uint64_t groups, void* out_dev);
+  // the same groups as normalised device generators (C::Gen), the layout of Handle::ptable
+  void (*partition_gens)(const EngineCtx&, const void* gens, uint64_t n, unsigned w,
+                         uint64_t first_group, uint64_t groups, void* out_gens);
 };
 extern const CurveVTable kVTableEd25519, kVTableBls12381, kVTableBn254, kVTableGrumpkin;
 

@@ -13,8 +13,12 @@
 //       the inversion tree of batch_affine.cuh (denominator 1 for Z = 0, the Weierstrass identity);
 //   PartitionStoreBody writes the affine coordinates (ed25519: also T = x y) in the compact layout,
 //       the identity encoding for Z = 0.
+// PartitionGenStoreBody writes the same entries in the curve's device generator layout (C::Gen, Z = 1)
+// instead, for a table kept on a handle and read by partition_msm.cuh.
 // The caller splits a table into chunks of whole groups; the scratch lives for one chunk only.
 #pragma once
+#include <type_traits>
+
 #include "batch_affine.cuh"
 
 namespace b200 {
@@ -55,11 +59,20 @@ template <class C> struct PartitionStoreBody {
   }
 };
 
+template <class C> struct PartitionGenStoreBody {
+  static constexpr int kBlock = 128;
+  const typename C::Point* pts;
+  const typename C::F::E* zinv;  // inverted denominators
+  typename C::Gen* out;
+  B200_HD void operator()(u64 i) const { C::normalized_gen(out[i], pts[i], zinv[i]); }
+};
+
 // groups [first_group, first_group + groups) of the partition table of width w over n generators
-// (device generator layout) -> compact ABI entries at `out`
-template <class C>
+// (device generator layout) -> compact ABI entries (Out = unsigned char) or normalised device
+// generators (Out = C::Gen) at `out`
+template <class C, class Out>
 inline void build_partition_table(stream_t s, const typename C::Gen* gens, u64 n, u32 w,
-                                  u64 first_group, u64 groups, unsigned char* out) {
+                                  u64 first_group, u64 groups, Out* out) {
   typedef typename C::Point Point;
   typedef typename C::F::E E;
   const u64 entries = groups << w;
@@ -70,7 +83,10 @@ inline void build_partition_table(stream_t s, const typename C::Gen* gens, u64 n
   for (u32 j = 0; j < w; ++j)
     launch(PartitionRoundBody<C>{gens, pts, den, n, first_group, w, j}, groups << j, s);
   batch_invert<typename C::F>(s, den, entries);
-  launch(PartitionStoreBody<C>{pts, den, out}, entries, s);
+  if constexpr (std::is_same<Out, unsigned char>::value)
+    launch(PartitionStoreBody<C>{pts, den, out}, entries, s);
+  else
+    launch(PartitionGenStoreBody<C>{pts, den, out}, entries, s);
   dev_free(den, s);
   dev_free(pts, s);
 }

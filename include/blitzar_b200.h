@@ -247,6 +247,16 @@ void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const v
  * sxt_multiexp_handle_new_from_file and by this library's. Synchronises before returning. */
 void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle* handle,
                                                 const char* filename, unsigned window_width);
+/* Attaches to the handle the partition table of width window_width (1..24; 0 = the reference's
+ * default, BLITZAR_PARTITION_WINDOW_WIDTH, else 16) over its generators, kept in HBM: 2^w subset sums
+ * per group of w generators (per shard with BLITZAR_B200_DEVICES). Fixed-base calls over the handle
+ * then answer the outputs that are cheaper that way (narrow widths) by table lookups. Replaces a
+ * table attached before. Returns the width attached, or 0 when the table would take more than 40 %
+ * of the free HBM; the handle then has no table and works as before. Synchronises. */
+unsigned b200_multiexp_handle_add_partition_table(struct sxt_multiexp_handle* handle,
+                                                  unsigned window_width);
+/* Width of the handle's partition table, or 0 when it has none. */
+unsigned b200_multiexp_handle_partition_window(const struct sxt_multiexp_handle* handle);
 /* Self-test of the warp-cooperative (lane-sliced) field arithmetic of the tail kernels against the
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
