@@ -62,7 +62,8 @@ def build_emul():
     prefix = os.path.join(edir, "emul_prefix.h")
     flags = ["g++", "-std=c++17", "-O1", "-DB200_EMULATE", "-fPIC", "-w", "-include", prefix]
     jobs, objs = [], []
-    harness = ["emul.cpp", "ptable_emul.cpp", "offsets_emul.cpp", "partition_msm_emul.cpp"]
+    harness = ["emul.cpp", "ptable_emul.cpp", "offsets_emul.cpp", "partition_msm_emul.cpp",
+               "normalize_emul.cpp"]
     for u in [x for x in UNITS if x.startswith("curve_")] + harness:
         src = os.path.join(edir if u in harness else CSRC, u)
         obj = os.path.join(objdir, u.rsplit(".", 1)[0] + ".o")

@@ -68,6 +68,8 @@ EngineCtx ctx_of(const State& st) {
     c.opt.scatter_window_major = (u32)std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_SORT"))  // 0 atomic, 1 binned (large), 2 binned
     c.opt.sort_path = (u32)std::atoi(env);
+  if (const char* env = std::getenv("BLITZAR_B200_NORMALIZE_GENS"))  // 0 = keep the caller's Z
+    c.opt.normalize_gens = (u32)std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_PAIR_LEVELS"))  // batch-affine levels (-1 = auto)
     c.opt.pair_levels = std::atoi(env);
   if (const char* env = std::getenv("BLITZAR_B200_PAIR_BATCH"))

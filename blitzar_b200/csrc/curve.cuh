@@ -241,14 +241,33 @@ struct Ed25519 {
     r = o;
   }
 
+  // a normalised generator (Z = 1) without a load of its Z2 field, which is the constant 2
+  static B200_HD Gen load_unit_gen(const Gen* src) {
+    Gen g;
+    g.YpX = src->YpX;
+    g.YmX = src->YmX;
+    g.T2d = src->T2d;
+    g.Z2 = F::zero();
+    g.Z2.l[0] = 2;
+    return g;
+  }
+
   // sxt_ristretto255 { u64 X[5], Y[5], Z[5], T[5] }
-  static B200_HD void load_gen_abi(Gen& g, const void* src) {
+  static B200_HD void load_point_abi(Point& p, const void* src) {
     const u64* s = (const u64*)src;
-    Point p;
     F::from_radix51(p.X, s);
     F::from_radix51(p.Y, s + 5);
     F::from_radix51(p.Z, s + 10);
     F::from_radix51(p.T, s + 15);
+  }
+  static B200_HD fe load_abi_z(const void* src) {
+    fe z;
+    F::from_radix51(z, (const u64*)src + 10);
+    return z;
+  }
+  static B200_HD void load_gen_abi(Gen& g, const void* src) {
+    Point p;
+    load_point_abi(p, src);
     point_to_gen(g, p);
   }
   static B200_HD void load_proj_abi(Gen& g, const void* src) { load_gen_abi(g, src); }

@@ -76,6 +76,7 @@ template <class C> struct CurveOps {
     bool builtin;  // generate g(offset + i) instead of converting `raw`
     range_wait_fn wait;
     void* wait_user;
+    u32* invalid = nullptr;  // non-null: normalise the generators to Z = 1 (ingest_normalized)
     bool pending = false;  // an ingestion is running on the second stream
     void before_range(u64 begin, u64 end) override {
       if (end > n)
@@ -85,10 +86,18 @@ template <class C> struct CurveOps {
       if (wait)
         wait(wait_user, begin, end);
       if (raw) {
-        // the sort of this range reads only scalars: the (HBM-bound) ingestion runs beside it on a
-        // second stream and is joined right before the first kernel that gathers generators
+        // the sort of this range reads only scalars: the ingestion runs beside it on a second
+        // stream and is joined right before the first kernel that gathers generators
         stream_t aux = aux_stream();
         stream_follow(aux, ctx->s);
+        if constexpr (C::kCurveId == kRistretto255) {
+          if (invalid) {
+            ingest_normalized(aux, raw + begin * C::kAbiGenBytes, gens + begin, IngestMap{},
+                              end - begin, invalid);
+            pending = true;
+            return;
+          }
+        }
         launch(IngestBody<C, false>{raw + begin * C::kAbiGenBytes, gens + begin}, end - begin, aux);
         pending = true;
       } else if (builtin) {
@@ -120,6 +129,7 @@ template <class C> struct CurveOps {
     Gen* gens;                 // the packed device generators
     range_wait_fn wait;
     void* wait_user;
+    u32* invalid = nullptr;  // non-null: normalise the generators to Z = 1 (ingest_normalized)
     bool pending = false;  // an ingestion is running on the second stream
     void before_range(u64 begin, u64 end) override {
       end = std::min<u64>(end, layout->max_n);
@@ -143,8 +153,16 @@ template <class C> struct CurveOps {
         stream_follow(on, ctx->s);
       const u64* staged = (const u64*)stage_to_device(on, block.data(), block.size() * sizeof(u64));
       const GenPieces p{staged, staged + np + 1, staged + 2 * np + 1, (u32)np};
+      bool normalized = false;
+      if constexpr (C::kCurveId == kRistretto255) {
+        if (raw && invalid) {
+          ingest_normalized(on, raw, gens, IngestMap{p}, block[np], invalid);
+          normalized = true;
+        }
+      }
       if (raw) {
-        launch(IngestPiecesBody<C>{raw, gens, p}, block[np], on);
+        if (!normalized)
+          launch(IngestPiecesBody<C>{raw, gens, p}, block[np], on);
         pending = true;
       } else if constexpr (C::kCurveId == kRistretto255) {
         launch(BuiltinPiecesBody{gens, p}, block[np], on);
@@ -231,9 +249,29 @@ template <class C> struct CurveOps {
         hook.builtin = true;
     }
     std::vector<ColumnDesc> cols = columns_of(d, num);
-    commit_columns(ctx, out_commitments, out_partials, cols, gens_ptr,
+    const Normalizing norm(ctx, n && generators_dev, &hook.invalid);
+    commit_columns(norm.ctx, out_commitments, out_partials, cols, gens_ptr,
                    n && !generators_dev && !hook.builtin, num_ranges, &hook);
   }
+  // Caller generators of ed25519 are normalised at ingestion (ingest_normalized) unless
+  // opt.normalize_gens is 0. Only then is the call's Z = 0 flag allocated and zeroed (*hook_invalid),
+  // and `ctx` runs the gathering level on Z = 1 generators unless that flag gets set.
+  struct Normalizing {
+    EngineCtx ctx;
+    u32* flag = nullptr;
+    Normalizing(const EngineCtx& c, bool ingests, u32** hook_invalid) : ctx(c) {
+      if (C::kCurveId != kRistretto255 || !ingests || !c.opt.normalize_gens)
+        return;
+      flag = (u32*)dev_alloc(sizeof(u32), c.s);
+      dev_zero(flag, sizeof(u32), c.s);
+      *hook_invalid = flag;
+      ctx.opt.gens_normalized = 1u;
+      ctx.opt.unit_veto = flag;
+    }
+    ~Normalizing() { dev_free(flag, ctx.s); }
+    Normalizing(const Normalizing&) = delete;
+    Normalizing& operator=(const Normalizing&) = delete;
+  };
 
   // commit_device with a generator start per column: row i of column j pairs with generator
   // offsets[j] + i (offsets null = all 0). The generators the columns use are laid out by GenLayout;
@@ -261,7 +299,8 @@ template <class C> struct CurveOps {
     std::vector<ColumnDesc> cols = columns_of(d, num);
     for (uint32_t j = 0; j < num; ++j)  // built-in array: generator g sits at position g
       cols[j].gen_base = builtin_table && d[j].n && offsets ? (u32)offsets[j] : layout.base[j];
-    commit_columns(ctx, out_commitments, out_partials, cols,
+    const Normalizing norm(ctx, layout.total && generators_dev, &hook.invalid);
+    commit_columns(norm.ctx, out_commitments, out_partials, cols,
                    builtin_table ? (const Gen*)ctx.builtin : gens.p, builtin_table, num_ranges,
                    &hook);
   }

@@ -26,7 +26,11 @@ struct MsmOptions {
   int range_skew = 0;   // piece schedule of a multi-range call (range_begin); set by the host layer
   u32 uniform_add = 2;  // gathering level: runs start from the identity (no divergent start path);
                         // 0 off, 1 on, 2 = ed25519 only
-  u32 gens_normalized = 0;  // set per call: the generator array is a fixed-base table (Z = 1 entries)
+  u32 gens_normalized = 0;  // set per call: the generator array has Z = 1 entries (fixed-base table,
+                            // or caller generators normalised at ingestion)
+  const u32* unit_veto = nullptr;  // set per call with gens_normalized: device flag, non-zero = the
+                                   // ingestion met Z = 0 and left the generators unnormalised
+  u32 normalize_gens = 1;  // ed25519 caller generators are normalised to Z = 1 at ingestion
   u32 lane_tail = 1;  // warp-cooperative (lane-sliced) Horner / encoding kernels for ed25519
   u32 scatter_window_major = 0;  // scatter with one thread per (window, term), window-major
   // bucket sort of the entries: 0 = atomic count + scan + scatter; 1 = binned sort (msm.cuh) for

@@ -618,11 +618,28 @@ inline void binned_sort(stream_t s, const ColumnDesc* d_cols, const u64* d_col_s
 }
 #endif
 
+// p[0 .. n) = identity, one 16-byte store per thread: consecutive threads write consecutive 16 bytes,
+// so every store instruction of a warp covers 512 contiguous bytes (a thread per point strides the
+// warp's stores by the point size and leaves every sector partially written)
 template <class C> struct FillIdentityBody {
   static constexpr int kBlock = 256;
-  typename C::Point* p;
-  B200_HD void operator()(u64 t) const { p[t] = C::identity(); }
+  static constexpr u32 kChunks = sizeof(typename C::Point) / 16;
+  static_assert(sizeof(typename C::Point) % 16 == 0, "points are made of 16-byte aligned fields");
+  uint4* p;
+  B200_HD void operator()(u64 t) const {
+    const typename C::Point id = C::identity();
+    const u32 k = (u32)(t % kChunks);
+    uint4 v = ((const uint4*)&id)[0];
+#pragma unroll
+    for (u32 j = 1; j < kChunks; ++j)  // constant indices: the identity stays in registers
+      if (j == k)
+        v = ((const uint4*)&id)[j];
+    p[t] = v;
+  }
 };
+template <class C> inline void fill_identity(stream_t s, typename C::Point* p, u64 n) {
+  launch(FillIdentityBody<C>{(uint4*)p}, n * FillIdentityBody<C>::kChunks, s);
+}
 
 // buckets[k] += scratch[k] for every bucket the current generator range touched (bucket_end = the
 // range's cursor array after the scatter). A later range accumulates into its own scratch array and
@@ -652,14 +669,21 @@ template <class C> struct MergeBucketsBody {
 // every other one, so that a run boundary costs the lanes that hit it only a bucket store and a reset
 // instead of a separate generator-to-point conversion path (one more multiplication by a constant) that
 // the rest of the warp waits for; the price is a full addition for the first element of every run.
-template <class C, bool kGather, class X = SeqExec, bool kUniform = false> struct AccumulateBody {
+// kUnitZ (gathering level, ed25519 only): every generator is normalised (Z = 1: a fixed-base table, or
+// caller generators normalised at ingestion), so an addition takes 7 multiplications and the gather
+// never loads Gen::Z2 (96 of the 128 bytes). unit_veto, when set, is a device flag read once at
+// entry: non-zero means the ingestion met Z = 0 and left the generators as they came, and the
+// 8-multiplication path over the whole Gen runs instead.
+template <class C, bool kGather, class X = SeqExec, bool kUniform = false, bool kUnitZ = false>
+struct AccumulateBody {
   static constexpr int kBlock = 128;
   // register cap: 168 (3 blocks/SM) for 8-limb fields; 12-limb bls12-381 keeps 255 (2 blocks/SM)
   static constexpr int kMinBlocks = !kGather ? 1 : (C::F::N > 8 ? 2 : 3);
   typedef typename C::Point Point;
+  typedef typename C::Gen Gen;
   const u32* keys;                 // level >= 2
   const u64* entries;              // level 1: (key << 32) | (generator index << 1) | negate
-  const typename C::Gen* gens;     // level 1
+  const Gen* gens;                 // level 1
   const Point* pieces;             // level >= 2
   const u32* m_ptr;                // number of entries at this level (device)
   u32 K;
@@ -668,7 +692,7 @@ template <class C, bool kGather, class X = SeqExec, bool kUniform = false> struc
   u32* out_keys;
   Point* out_pieces;
   u32* out_m_ptr;
-  u32 unit_z;  // level 1: every generator is normalised (fixed-base table) — 7M additions on ed25519
+  const u32* unit_veto;  // kUnitZ: device flag, non-zero = run the 8-multiplication path; may be null
 
   // every bucket is written exactly once per generator range (a run strictly inside a chunk is
   // complete; split runs travel down the cascade and are written by the level that completes them)
@@ -691,6 +715,76 @@ template <class C, bool kGather, class X = SeqExec, bool kUniform = false> struc
         C::template add<X>(acc, acc, pieces[i]);
     }
   }
+  template <bool kUnit> B200_HD Gen load_gen(u32 idx) const {
+    if constexpr (kUnit)
+      return C::load_unit_gen(gens + idx);
+    else
+      return gens[idx];
+  }
+  // level 1: sums entries [b, e) of chunk t
+  template <bool kUnit>
+  B200_HD void gather_walk(u64 t, u64 b, u64 e, bool writer, u32& cur, Point& acc,
+                           bool& first_seg) const {
+    // software-pipelined gather: the generator of entry i+1 is loaded into registers before the
+    // addition of entry i starts, so the random 128-byte read overlaps ~1300 instructions of
+    // field arithmetic instead of stalling the warp on the long scoreboard
+    u64 ent = entries[b];
+    Gen g = load_gen<kUnit>((u32)ent >> 1);
+    cur = (u32)(ent >> 32);
+    struct {
+      Point p;
+      B200_HD void start(const Gen& g, bool negate) { C::gen_to_point(p, g, negate); }
+      B200_HD void add(const Gen& g, bool negate) {
+        C::template add_gen<X>(p, p, g, negate, kUnit);
+      }
+      B200_HD void get(Point& out) const { out = p; }
+    } ga;
+    for (u64 i = b; i < e; ++i) {
+      u64 ent_n = ent;
+      Gen g_n = g;
+      if (i + 1 < e) {
+        ent_n = entries[i + 1];
+        g_n = load_gen<kUnit>((u32)ent_n >> 1);
+      }
+      const u32 k = (u32)(ent >> 32);
+      const bool negate = ((u32)ent & 1u) != 0;
+      if (kUniform) {
+        if (i == b) {
+          ga.p = C::identity();
+        } else if (k != cur) {
+          ga.get(acc);
+          if (final_level || !first_seg) {
+            put_bucket(cur, acc, writer);
+          } else if (writer) {
+            out_keys[2 * t] = cur;
+            out_pieces[2 * t] = acc;
+          }
+          first_seg = false;
+          cur = k;
+          ga.p = C::identity();
+        }
+        ga.add(g, negate);
+      } else if (i == b) {
+        ga.start(g, negate);
+      } else if (k == cur) {
+        ga.add(g, negate);
+      } else {
+        ga.get(acc);
+        if (final_level || !first_seg) {
+          put_bucket(cur, acc, writer);
+        } else if (writer) {
+          out_keys[2 * t] = cur;
+          out_pieces[2 * t] = acc;
+        }
+        first_seg = false;
+        cur = k;
+        ga.start(g, negate);
+      }
+      ent = ent_n;
+      g = g_n;
+    }
+    ga.get(acc);
+  }
   B200_HD void operator()(u64 tid) const {
     const u64 t = tid / X::kLanes;
     const bool writer = (tid % X::kLanes) == 0;
@@ -706,67 +800,10 @@ template <class C, bool kGather, class X = SeqExec, bool kUniform = false> struc
     Point acc;
     bool first_seg = true;
     if (kGather) {
-      // software-pipelined gather: the generator of entry i+1 is loaded into registers before the
-      // addition of entry i starts, so the random 128-byte read overlaps ~1300 instructions of
-      // field arithmetic instead of stalling the warp on the long scoreboard
-      u64 ent = entries[b];
-      typename C::Gen g = gens[(u32)ent >> 1];
-      cur = (u32)(ent >> 32);
-      struct {
-        Point p;
-        bool unit;
-        B200_HD void start(const typename C::Gen& g, bool negate) { C::gen_to_point(p, g, negate); }
-        B200_HD void add(const typename C::Gen& g, bool negate) {
-          C::template add_gen<X>(p, p, g, negate, unit);
-        }
-        B200_HD void get(Point& out) const { out = p; }
-      } ga;
-      ga.unit = unit_z != 0;
-      for (u64 i = b; i < e; ++i) {
-        u64 ent_n = ent;
-        typename C::Gen g_n = g;
-        if (i + 1 < e) {
-          ent_n = entries[i + 1];
-          g_n = gens[(u32)ent_n >> 1];
-        }
-        const u32 k = (u32)(ent >> 32);
-        const bool negate = ((u32)ent & 1u) != 0;
-        if (kUniform) {
-          if (i == b) {
-            ga.p = C::identity();
-          } else if (k != cur) {
-            ga.get(acc);
-            if (final_level || !first_seg) {
-              put_bucket(cur, acc, writer);
-            } else if (writer) {
-              out_keys[2 * t] = cur;
-              out_pieces[2 * t] = acc;
-            }
-            first_seg = false;
-            cur = k;
-            ga.p = C::identity();
-          }
-          ga.add(g, negate);
-        } else if (i == b) {
-          ga.start(g, negate);
-        } else if (k == cur) {
-          ga.add(g, negate);
-        } else {
-          ga.get(acc);
-          if (final_level || !first_seg) {
-            put_bucket(cur, acc, writer);
-          } else if (writer) {
-            out_keys[2 * t] = cur;
-            out_pieces[2 * t] = acc;
-          }
-          first_seg = false;
-          cur = k;
-          ga.start(g, negate);
-        }
-        ent = ent_n;
-        g = g_n;
-      }
-      ga.get(acc);
+      if (kUnitZ && unit_veto && *unit_veto)
+        gather_walk<false>(t, b, e, writer, cur, acc, first_seg);
+      else
+        gather_walk<kUnitZ>(t, b, e, writer, cur, acc, first_seg);
     } else {
       cur = key_at(b);
       fetch(acc, b, true);
@@ -1091,6 +1128,252 @@ struct BuiltinPiecesBody {
     BuiltinGeneratorBody{gens + p.to[k], p.from[k]}(tid - p.start[k]);
   }
 };
+
+// ---- normalising ingestion (ed25519) ---------------------------------------------------------------
+// Caller generators come with any Z. Scaled by 1/Z (all four coordinates, so the projective point is
+// the same whatever its T) they have Z = 1 and 2Z = 2, and every bucket addition over them takes 7
+// multiplications instead of 8 (add_gen, unit_z) and gathers 96 bytes instead of 128
+// (AccumulateBody kUnitZ). A range of n generators is normalised by Montgomery's trick in two passes
+// around the inversion of the group products; thread j owns the generators j, j + T, j + 2T, ...
+// (T = ceil(n / kBatchGroup), so that a warp reads and writes consecutive generators):
+//   NormalizeUpBody:   reads only Z (40 of the 160 ABI bytes), writes the prefix products and the
+//                      group product
+//   the T group products are inverted (batch_invert; on CUDA NormalizeUpBlockBody and
+//                      NormalizeMidBody below, so that the whole normalisation is three launches)
+//   NormalizeDownBody: walks the group backwards, peeling 1/Z off the inverted product, and writes
+//                      the scaled generator in the device layout (IngestBody's only write)
+// Z = 0 is not a point: it counts as 1 in the products and sets *invalid. The down pass of a range
+// that finds *invalid set writes the generators unscaled, exactly as IngestBody, and the gathering
+// level, which reads the same flag, runs its 8-multiplication path over them.
+struct IngestMap {  // ingestion thread i: ABI generator src of `raw` -> device generator dst
+  GenPieces p;      // npieces == 0: src = dst = i
+  B200_HD void at(u64 i, u64& src, u64& dst) const {
+    if (p.npieces == 0) {
+      src = dst = i;
+      return;
+    }
+    const u32 k = column_of(p.start, p.npieces, i);
+    src = p.from[k] + (i - p.start[k]);
+    dst = p.to[k] + (i - p.start[k]);
+  }
+};
+constexpr u32 kNormBlock = 256;  // groups per block of the CUDA up pass
+struct NormalizeUpBody {
+  static constexpr int kBlock = 128;
+  typedef F25519 F;
+  const unsigned char* raw;
+  IngestMap map;
+  u64 n, T;
+  F::E* pre;   // [n]
+  F::E* prod;  // [T]
+  u32* invalid;
+  // prefix products of group j into pre; returns the group product
+  B200_HD F::E group(u64 j) const {
+    F::E z[kBatchGroup], acc = F::one();
+#pragma unroll
+    for (u32 k = 0; k < kBatchGroup; ++k) {  // all loads first: 8 reads in flight per thread
+      const u64 i = j + k * T;
+      z[k] = F::one();
+      if (i < n) {
+        u64 src, dst;
+        map.at(i, src, dst);
+        z[k] = Ed25519::load_abi_z(raw + src * Ed25519::kAbiGenBytes);
+      }
+    }
+#pragma unroll
+    for (u32 k = 0; k < kBatchGroup; ++k) {
+      const u64 i = j + k * T;
+      if (i >= n)
+        break;
+      if (F::is_zero(z[k])) {
+        *invalid = 1u;
+        z[k] = F::one();
+      }
+      pre[i] = acc;
+      F::mul(acc, acc, z[k]);
+    }
+    return acc;
+  }
+  B200_HD void operator()(u64 j) const { prod[j] = group(j); }
+};
+struct NormalizeDownBody {
+  static constexpr int kBlock = 128;
+  typedef F25519 F;
+  const unsigned char* raw;
+  IngestMap map;
+  u64 n, T;
+  const F::E* pre;
+  const F::E* prod;  // inverted: of every group, or (with ps) of every block of kNormBlock groups
+  const F::E* ps;    // null, or per group the product of the other groups of its block
+  const u32* invalid;
+  Ed25519::Gen* gens;
+  B200_HD void operator()(u64 j) const {
+    const bool scale = *invalid == 0;
+    F::E inv = prod[ps ? j / kNormBlock : j];
+    if (ps)
+      F::mul(inv, inv, ps[j]);
+    for (u32 k = kBatchGroup; k-- > 0;) {
+      const u64 i = j + k * T;
+      if (i >= n)
+        continue;
+      u64 src, dst;
+      map.at(i, src, dst);
+      Ed25519::Point p;
+      Ed25519::load_point_abi(p, raw + src * Ed25519::kAbiGenBytes);
+      if (scale) {  // no Z of the range is 0
+        F::E zi;
+        F::mul(zi, inv, pre[i]);
+        F::mul(inv, inv, p.Z);
+        F::mul(p.X, p.X, zi);
+        F::mul(p.Y, p.Y, zi);
+        F::mul(p.T, p.T, zi);
+        p.Z = F::one();
+      }
+      Ed25519::Gen g;
+      Ed25519::point_to_gen(g, p);
+      gens[dst] = g;
+    }
+  }
+};
+#ifdef B200_BINNED_SORT
+// CUDA: the T group products are inverted in two more kernels instead of batch_invert's tree (a
+// chain of ~10 small launches that, beside the sort's large blocks, each wait for a free SM):
+//   NormalizeUpBlockBody: the up pass, plus per block of kNormBlock groups the exclusive prefix and
+//                         suffix products of the group products (warp shuffles): ps[j] = product of
+//                         the other groups of the block, prod[b] = the block's product
+//   NormalizeMidBody:     one block inverts the blocks' products in place (Montgomery's trick over
+//                         chunks, the same scans across the chunks, one inversion)
+//   NormalizeDownBody:    1 / (group product) = prod[b] * ps[j]
+__device__ __forceinline__ F25519::E shfl_up_fe(const F25519::E& a, u32 d) {
+  F25519::E r;
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    r.l[k] = __shfl_up_sync(0xffffffffu, a.l[k], d);
+  return r;
+}
+__device__ __forceinline__ F25519::E shfl_down_fe(const F25519::E& a, u32 d) {
+  F25519::E r;
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    r.l[k] = __shfl_down_sync(0xffffffffu, a.l[k], d);
+  return r;
+}
+// exclusive prefix (P) and suffix (S) products of x over the kBlock threads of the block, and the
+// block's product (every thread); ws: kBlock / 32 elements of shared memory
+template <int kBlock>
+__device__ void block_prefix_suffix(const F25519::E& x, F25519::E& P, F25519::E& S,
+                                    F25519::E& total, F25519::E* ws) {
+  typedef F25519 F;
+  const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  F::E inc = x, sinc = x;
+#pragma unroll
+  for (u32 d = 1; d < 32; d <<= 1) {
+    const F::E y = shfl_up_fe(inc, d), z = shfl_down_fe(sinc, d);
+    if (lane >= d)
+      F::mul(inc, inc, y);
+    if (lane + d < 32)
+      F::mul(sinc, sinc, z);
+  }
+  F::E pe = shfl_up_fe(inc, 1), se = shfl_down_fe(sinc, 1);
+  if (lane == 0)
+    pe = F::one();
+  if (lane == 31) {
+    se = F::one();
+    ws[warp] = inc;
+  }
+  __syncthreads();
+  F::E before = F::one(), after = F::one();
+  for (u32 w = 0; w < kBlock / 32; ++w) {
+    if (w < warp)
+      F::mul(before, before, ws[w]);
+    else if (w > warp)
+      F::mul(after, after, ws[w]);
+  }
+  F::mul(P, before, pe);
+  F::mul(S, se, after);
+  F::mul(total, before, ws[warp]);
+  F::mul(total, total, after);
+  __syncthreads();  // ws may be reused right away
+}
+struct NormalizeUpBlockBody {
+  static constexpr int kBlock = kNormBlock;
+  typedef F25519 F;
+  NormalizeUpBody up;
+  F::E* ps;    // [T]
+  F::E* prod;  // [blocks]
+  __device__ void run(u32 b, unsigned char*) const {
+    __shared__ F::E ws[kBlock / 32];
+    const u64 j = (u64)b * kBlock + threadIdx.x;
+    const F::E g = j < up.T ? up.group(j) : F::one();
+    F::E P, S, total;
+    block_prefix_suffix<kBlock>(g, P, S, total, ws);
+    if (j < up.T)
+      F::mul(ps[j], P, S);
+    if (threadIdx.x == 0)
+      prod[b] = total;
+  }
+};
+struct NormalizeMidBody {
+  static constexpr int kBlock = 1024;
+  typedef F25519 F;
+  F::E* vals;  // [m], inverted in place
+  F::E* pre;   // [m] scratch
+  u64 m;
+  __device__ void run(u32, unsigned char*) const {
+    __shared__ F::E ws[kBlock / 32];
+    __shared__ F::E inv_total;
+    const u64 per = (m + kBlock - 1) / kBlock, lo = min((u64)threadIdx.x * per, m),
+              hi = min(lo + per, m);
+    F::E c = F::one();
+    for (u64 k = lo; k < hi; ++k) {
+      pre[k] = c;
+      F::mul(c, c, vals[k]);
+    }
+    F::E P, S, total;
+    block_prefix_suffix<kBlock>(c, P, S, total, ws);
+    if (threadIdx.x == 0)
+      F::invert(inv_total, total);
+    __syncthreads();
+    F::E inv;  // 1 / c
+    F::mul(inv, inv_total, P);
+    F::mul(inv, inv, S);
+    for (u64 k = hi; k-- > lo;) {
+      const F::E v = vals[k];
+      F::mul(vals[k], inv, pre[k]);
+      F::mul(inv, inv, v);
+    }
+  }
+};
+#endif
+// IngestBody (map without pieces) / IngestPiecesBody of n generators, normalised; enqueued on s.
+// *invalid is zeroed by the caller once per call and set here when a generator has Z = 0.
+inline void ingest_normalized(stream_t s, const unsigned char* raw, Ed25519::Gen* gens,
+                              const IngestMap& map, u64 n, u32* invalid) {
+  typedef F25519::E fe;
+  if (n == 0)
+    return;
+  const u64 T = (n + kBatchGroup - 1) / kBatchGroup;
+  fe* pre = (fe*)dev_alloc(n * sizeof(fe), s);
+  const NormalizeUpBody up{raw, map, n, T, pre, nullptr, invalid};
+#ifdef B200_BINNED_SORT
+  const u64 blocks = (T + kNormBlock - 1) / kNormBlock;
+  fe* ps = (fe*)dev_alloc((T + 2 * blocks) * sizeof(fe), s);
+  fe* prod = ps + T;
+  launch_blocks(NormalizeUpBlockBody{up, ps, prod}, blocks, 0, s);
+  launch_blocks(NormalizeMidBody{prod, prod + blocks, blocks}, 1, 0, s);
+  launch(NormalizeDownBody{raw, map, n, T, pre, prod, ps, invalid, gens}, T, s);
+  dev_free(ps, s);
+#else
+  fe* prod = (fe*)dev_alloc(T * sizeof(fe), s);
+  NormalizeUpBody u = up;
+  u.prod = prod;
+  launch(u, T, s);
+  batch_invert<F25519>(s, prod, T);
+  launch(NormalizeDownBody{raw, map, n, T, pre, prod, nullptr, invalid, gens}, T, s);
+  dev_free(prod, s);
+#endif
+  dev_free(pre, s);
+}
 // result canonicalisation
 template <class C, bool kCommit> struct StoreBody {
   static constexpr int kBlock = 32;
@@ -1346,10 +1629,12 @@ struct RangeHook {
 };
 
 // Chunk walk of `walk` into `target`, then the cascade over its pieces (appended to to_free) on `tail`
-// when it differs from s. Returns the stream of the last level.
+// when it differs from s. Returns the stream of the last level. unit: walk.gens are normalised
+// (Z = 1) unless *unit_veto is set on the device (AccumulateBody kUnitZ).
 template <class C>
-stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, u32 unit_z,
-                    typename C::Point* target, const MsmOptions& opt, std::vector<void*>& to_free) {
+stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, bool unit,
+                    const u32* unit_veto, typename C::Point* target, const MsmOptions& opt,
+                    std::vector<void*>& to_free) {
   typedef typename C::Point Point;
   // a chunk of K entries leaves 2 pieces, so K must exceed 2 for the cascade to shrink
   // at C2, K = 64 trims the cascade more than it costs the first level
@@ -1370,14 +1655,27 @@ stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, u32 
       // start is free, so the extra addition loses
       const bool uniform =
           opt.uniform_add == 2 ? C::kCurveId == kRistretto255 : opt.uniform_add != 0;
-      if (uniform)
+      // normalised generators change the addition on ed25519 only (Weierstrass generators are affine)
+      constexpr bool kEd = C::kCurveId == kRistretto255;
+      const bool unit_path = kEd && unit;
+      if (uniform && unit_path)
+        launch(AccumulateBody<C, true, SeqExec, true, kEd>{nullptr, walk.entries, walk.gens, nullptr,
+                                                            walk.m_ptr, K, final_level, target,
+                                                            out_keys, out_pieces, out_m, unit_veto},
+               T, s);
+      else if (uniform)
         launch(AccumulateBody<C, true, SeqExec, true>{nullptr, walk.entries, walk.gens, nullptr,
                                                       walk.m_ptr, K, final_level, target, out_keys,
-                                                      out_pieces, out_m, unit_z},
+                                                      out_pieces, out_m, nullptr},
+               T, s);
+      else if (unit_path)
+        launch(AccumulateBody<C, true, SeqExec, false, kEd>{nullptr, walk.entries, walk.gens, nullptr,
+                                                             walk.m_ptr, K, final_level, target,
+                                                             out_keys, out_pieces, out_m, unit_veto},
                T, s);
       else
         launch(AccumulateBody<C, true>{nullptr, walk.entries, walk.gens, nullptr, walk.m_ptr, K,
-                                       final_level, target, out_keys, out_pieces, out_m, unit_z},
+                                       final_level, target, out_keys, out_pieces, out_m, nullptr},
                T, s);
       KernelTimer::get().end(s);
       if (tail != s)
@@ -1385,11 +1683,12 @@ stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, u32 
       cs = tail;
     } else if (T <= opt.quad_threshold) {
       launch(AccumulateBody<C, false, QuadExec>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr,
-                                                K, final_level, target, out_keys, out_pieces, out_m, 0u},
+                                                K, final_level, target, out_keys, out_pieces, out_m,
+                                                nullptr},
              T * QuadExec::kLanes, cs);
     } else {
       launch(AccumulateBody<C, false>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr, K,
-                                      final_level, target, out_keys, out_pieces, out_m, 0u},
+                                      final_level, target, out_keys, out_pieces, out_m, nullptr},
              T, cs);
     }
     if (final_level)
@@ -1452,8 +1751,9 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
   }
   typedef typename C::Point Point;  // later ranges: own bucket array, merged into the shared one below
   Point* target = add_into ? (Point*)dev_alloc(nkeys * sizeof(Point), s) : d_buckets;
-  const u32 unit_z = (walk.gens == gens && opt.gens_normalized) ? 1u : 0u;
-  const stream_t cs = chunk_walk<C>(s, tail, walk, sorted.d_m, unit_z, target, opt, to_free);
+  const bool unit = walk.gens == gens && opt.gens_normalized;
+  const stream_t cs =
+      chunk_walk<C>(s, tail, walk, sorted.d_m, unit, opt.unit_veto, target, opt, to_free);
   // What the later levels and the merge read on cs (pieces, keys, d_m, counts, starts) is freed on cs:
   // freed on s, it could go to the next range's allocations while cs still reads it. So are the last
   // pair level's points and entries. The sorted entries and the staged columns are read on s only.
@@ -1557,11 +1857,11 @@ void msm_run(stream_t s, const typename C::Gen* gens, std::vector<ColumnDesc> co
   if (plan.total_terms == 0 || plan.total_windows == 0) {
     if (hook)
       hook->before_range(0, plan.max_n);
-    launch(FillIdentityBody<C>{out}, plan.ncols, s);
+    fill_identity<C>(s, out, plan.ncols);
     return;
   }
   Point* d_buckets = (Point*)dev_alloc(plan.nkeys * sizeof(Point), s);
-  launch(FillIdentityBody<C>{d_buckets}, plan.nkeys, s);
+  fill_identity<C>(s, d_buckets, plan.nkeys);
   u32* d_window_used = (u32*)dev_alloc(plan.total_windows * sizeof(u32), s);
   dev_zero(d_window_used, plan.total_windows * sizeof(u32), s);
   if (num_ranges < 1)
