@@ -53,8 +53,9 @@ def build_product(verbose=False):
 
 
 def build_emul():
-    """CPU emulation harness (test infrastructure): the per-curve units of the product compiled as
-    host C++ (-DB200_EMULATE, tests/emul/emul_prefix.h force-included), in parallel."""
+    """CPU emulation harness (test infrastructure): the per-curve units of the product and the
+    harness's own sources (tests/emul/*.cpp) compiled as host C++ (-DB200_EMULATE,
+    tests/emul/emul_prefix.h force-included), in parallel."""
     edir = os.path.join(ROOT, "tests", "emul")
     out = os.path.join(edir, "libb200_emul.so")
     objdir = os.path.join(edir, "obj")
@@ -62,10 +63,11 @@ def build_emul():
     prefix = os.path.join(edir, "emul_prefix.h")
     flags = ["g++", "-std=c++17", "-O1", "-DB200_EMULATE", "-fPIC", "-w", "-include", prefix]
     jobs, objs = [], []
-    harness = ["emul.cpp", "ptable_emul.cpp", "offsets_emul.cpp", "partition_msm_emul.cpp",
-               "normalize_emul.cpp"]
-    for u in [x for x in UNITS if x.startswith("curve_")] + harness:
-        src = os.path.join(edir if u in harness else CSRC, u)
+    harness = sorted(f for f in os.listdir(edir) if f.endswith(".cpp"))
+    srcs = [os.path.join(CSRC, u) for u in UNITS if u.startswith("curve_")] + \
+        [os.path.join(edir, f) for f in harness]
+    for src in srcs:
+        u = os.path.basename(src)
         obj = os.path.join(objdir, u.rsplit(".", 1)[0] + ".o")
         objs.append(obj)
         if _newer(obj, [src, prefix] + _headers()):

@@ -155,21 +155,6 @@ void require_init(const char* fn) {
   B200_CUDA(cudaSetDevice(g_state.device));
 }
 
-const CurveVTable& vt(unsigned curve_id) {
-  switch (curve_id) {
-  case SXT_CURVE_RISTRETTO255:
-    return kVTableEd25519;
-  case SXT_CURVE_BLS_381:
-    return kVTableBls12381;
-  case SXT_CURVE_BN_254:
-    return kVTableBn254;
-  case SXT_CURVE_GRUMPKIN:
-    return kVTableGrumpkin;
-  default:
-    die("unsupported curve id", __FILE__, __LINE__);
-  }
-}
-
 
 // Host-to-device upload of PAGEABLE caller memory. A plain cudaMemcpyAsync from pageable memory is
 // staged by the driver on one thread, at the copy rate of one core.
@@ -348,7 +333,7 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
                const sxt_sequence_descriptor* d, const void* generators,
                uint64_t offset_generators, void* out_partials_dev = nullptr,
                const uint64_t* offsets = nullptr) {
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   StageRange nvtx("commit (host buffers)");
   cudaStream_t s = st.stream, sc = st.copy_stream;
   uint64_t n = longest_column(d, num);
@@ -587,7 +572,7 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
     B200_REQUIRE(generators != nullptr, "generators == nullptr");
   if (offsets)
     (void)GenLayout(d, num, offsets);  // validates the offsets before any thread starts
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   const size_t stride = V.abi_commit_bytes;
   const size_t devices = g_workers.size() + 1;
   if (devices <= 1 || out_partials_dev) {
@@ -674,7 +659,7 @@ struct HandleSet {
 // in_memory_partition_table_accessor_utility.h:41-79).
 Handle* shard_new(const State& st, unsigned curve_id, const void* generators, unsigned n,
                   bool device_resident, unsigned compact_window, size_t compact_bytes) {
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   cudaStream_t s = st.stream;
   Handle* h = new Handle{curve_id, n, nullptr};
   h->window_bits = choose_table_window(n, V.gen_bytes);
@@ -724,7 +709,7 @@ uint64_t partition_chunk_groups(const CurveVTable& V, unsigned w) {
 // chunks of whole groups. The table may take at most 40 % of the free HBM, as the fixed-base tables
 // do (choose_table_window); false, and no table, when it does not fit.
 bool shard_add_partition_table(const State& st, Handle* h, unsigned w) {
-  const CurveVTable& V = vt(h->curve_id);
+  const CurveVTable& V = curve_vtable(h->curve_id);
   cudaStream_t s = st.stream;
   stream_sync(s);
   B200_CUDA(cudaFree(h->ptable));
@@ -779,7 +764,7 @@ unsigned handle_add_partition_table(HandleSet* hs, unsigned window_width) {
 HandleSet* handle_new(unsigned curve_id, const void* generators, unsigned n,
                       bool device_resident = false, unsigned compact_window = 0,
                       size_t compact_bytes = 0) {
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   HandleSet* hs = new HandleSet;
   hs->curve_id = curve_id;
   hs->n = n;
@@ -825,7 +810,7 @@ struct FixedCall {
 void fixed_on(const State& st, void* res, const Handle* h, const FixedCall& c, unsigned lo,
               const uint8_t* scalars, void* out_partials_dev) {
   cudaStream_t s = st.stream;
-  const CurveVTable& V = vt(h->curve_id);
+  const CurveVTable& V = curve_vtable(h->curve_id);
   const unsigned hi = std::min<uint64_t>((uint64_t)lo + h->n, c.rows);
   const unsigned rows = hi > lo ? hi - lo : 0;
   std::vector<unsigned> lens;
@@ -869,7 +854,7 @@ void fixed_host(void* res, const HandleSet* hs, int mode, unsigned element_num_b
     fixed_on(g_state, res, hs->shards[0], c, 0, scalars, out_partials_dev);
     return;
   }
-  const CurveVTable& V = vt(hs->curve_id);
+  const CurveVTable& V = curve_vtable(hs->curve_id);
   const size_t pbytes = (size_t)num_outputs * V.point_bytes;
   void* gather = g_gather.ensure(parts * pbytes);
   on_devices(parts, [&, hs, scalars, pbytes, gather](size_t p) {
@@ -1111,7 +1096,7 @@ void sxt_multiexp_handle_write_to_file(const struct sxt_multiexp_handle* handle,
   require_init("sxt_multiexp_handle_write_to_file");
   const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
   B200_REQUIRE(h && filename, "null handle or filename");
-  const CurveVTable& V = vt(h->curve_id);
+  const CurveVTable& V = curve_vtable(h->curve_id);
   size_t bytes = (size_t)h->n * V.abi_proj_bytes;
   std::vector<unsigned char> host(bytes);
   on_devices(h->shards.size(), [&, h](size_t p) {
@@ -1147,7 +1132,7 @@ struct sxt_multiexp_handle* sxt_multiexp_handle_new_from_file(unsigned curve_id,
     // this library's table is rebuilt from them on the device (groups padded with the identity stay
     // identities, as in the reference).
     const unsigned w = hdr[0];
-    const size_t esz = vt(curve_id).abi_compact_bytes;
+    const size_t esz = curve_vtable(curve_id).abi_compact_bytes;
     B200_REQUIRE(w >= 1 && w <= 24, "not a handle file (bad window width)");
     std::fseek(f, 0, SEEK_END);
     const size_t bytes = (size_t)std::ftell(f) - sizeof(uint32_t);
@@ -1164,7 +1149,7 @@ struct sxt_multiexp_handle* sxt_multiexp_handle_new_from_file(unsigned curve_id,
   B200_REQUIRE(std::fread(hdr + 1, 3 * sizeof(uint32_t), 1, f) == 1, "short handle file");
   B200_REQUIRE(hdr[1] == 1u, "unsupported blitzar_b200 handle file version");
   B200_REQUIRE(hdr[2] == curve_id, "handle file is for another curve");
-  size_t bytes = (size_t)hdr[3] * vt(curve_id).abi_proj_bytes;
+  size_t bytes = (size_t)hdr[3] * curve_vtable(curve_id).abi_proj_bytes;
   std::vector<unsigned char> host(bytes);
   B200_REQUIRE(bytes == 0 || std::fread(host.data(), bytes, 1, f) == 1, "short handle file");
   std::fclose(f);
@@ -1209,7 +1194,7 @@ void b200_set_device(int device) {
   g_state.device = device;
 }
 unsigned long long b200_launch_count(void) { return LaunchCounter::value(); }
-unsigned b200_point_bytes(unsigned curve_id) { return vt(curve_id).point_bytes; }
+unsigned b200_point_bytes(unsigned curve_id) { return curve_vtable(curve_id).point_bytes; }
 void* b200_malloc(uint64_t bytes) {
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_malloc");
@@ -1271,8 +1256,9 @@ void b200_commit_device(unsigned curve_id, void* out_commitments, void* out_part
     return;
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_commit_device");
-  vt(curve_id).commit_device(ctx(), out_commitments, out_partials, num_sequences, descriptors,
-                             generators, offset_generators, 1, nullptr, nullptr);
+  curve_vtable(curve_id).commit_device(ctx(), out_commitments, out_partials, num_sequences,
+                                       descriptors, generators, offset_generators, 1, nullptr,
+                                       nullptr);
 }
 void b200_compute_pedersen_commitments_with_offsets(unsigned curve_id, void* commitments,
                                                     uint32_t num_sequences,
@@ -1289,7 +1275,7 @@ void b200_commit_device_with_offsets(unsigned curve_id, void* out_commitments, v
     return;
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_commit_device_with_offsets");
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   if (offsets)
     V.commit_device_offsets(ctx(), out_commitments, out_partials, num_sequences, descriptors,
                             generators, offsets, false, 1, nullptr, nullptr);
@@ -1333,7 +1319,7 @@ void b200_combine_partials_device(unsigned curve_id, void* out_commitments, cons
                                   uint32_t num_parts, uint32_t count) {
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_combine_partials_device");
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   DevBuf<unsigned char> sum((size_t)count * V.point_bytes, g_state.stream);
   V.sum_parts(ctx(), partials, num_parts, count, sum.p);
   V.store(ctx(), sum.p, out_commitments, count, true);
@@ -1343,7 +1329,7 @@ void b200_combine_partials_projective_device(unsigned curve_id, void* out_res,
                                              uint32_t count) {
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_combine_partials_projective_device");
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   DevBuf<unsigned char> sum((size_t)count * V.point_bytes, g_state.stream);
   V.sum_parts(ctx(), partials, num_parts, count, sum.p);
   V.store(ctx(), sum.p, out_res, count, false);
@@ -1367,8 +1353,9 @@ void b200_fixed_msm_device(void* out_res, void* out_partials,
     for (unsigned j = 0; j < num_outputs; ++j)
       rows = output_lengths[j] > rows ? output_lengths[j] : rows;
   }
-  vt(h->curve_id).fixed_device(ctx(), out_res, out_partials, h, mode, element_num_bytes,
-                               output_bit_table, output_lengths, num_outputs, rows, scalars);
+  curve_vtable(h->curve_id).fixed_device(ctx(), out_res, out_partials, h, mode, element_num_bytes,
+                                         output_bit_table, output_lengths, num_outputs, rows,
+                                         scalars);
 }
 void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, uint64_t n,
                                       uint64_t first, int projective) {
@@ -1377,13 +1364,13 @@ void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, u
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_synthetic_generators_device");
   B200_REQUIRE(out_generators != nullptr, "out_generators == nullptr");
-  vt(curve_id).synth_generators(ctx(), out_generators, n, first, projective != 0);
+  curve_vtable(curve_id).synth_generators(ctx(), out_generators, n, first, projective != 0);
 }
 void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const void* generators_dev,
                                  uint64_t n, unsigned window_width) {
   std::lock_guard<std::mutex> lock(g_mutex);
   require_init("b200_partition_table_device");
-  const CurveVTable& V = vt(curve_id);
+  const CurveVTable& V = curve_vtable(curve_id);
   const unsigned w = partition_window(window_width);
   if (n == 0)
     return;
@@ -1408,7 +1395,7 @@ void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle
   require_init("b200_multiexp_handle_write_partition_table");
   const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
   B200_REQUIRE(h && filename, "null handle or filename");
-  const CurveVTable& V = vt(h->curve_id);
+  const CurveVTable& V = curve_vtable(h->curve_id);
   const unsigned w = partition_window(window_width);
   cudaStream_t s = g_state.stream, sc = g_state.copy_stream;
   DevBuf<unsigned char> gens((size_t)(h->n ? h->n : 1) * V.gen_bytes, s);

@@ -237,6 +237,21 @@ struct CurveVTable {
 };
 extern const CurveVTable kVTableEd25519, kVTableBls12381, kVTableBn254, kVTableGrumpkin;
 
+inline const CurveVTable& curve_vtable(unsigned curve_id) {
+  switch (curve_id) {
+  case SXT_CURVE_RISTRETTO255:
+    return kVTableEd25519;
+  case SXT_CURVE_BLS_381:
+    return kVTableBls12381;
+  case SXT_CURVE_BN_254:
+    return kVTableBn254;
+  case SXT_CURVE_GRUMPKIN:
+    return kVTableGrumpkin;
+  default:
+    die("unsupported curve id", __FILE__, __LINE__);
+  }
+}
+
 // inner-product argument over ristretto255 (ipa.cuh); same contracts as the two sxt_* entry points
 void ipa_prove(const EngineCtx& ctx, uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value,
                uint8_t* transcript203, uint64_t n, uint64_t generators_offset,

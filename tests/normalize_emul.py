@@ -1,8 +1,5 @@
-"""Ristretto255 generators in scaled representations, and the Python side of the emulated normalising
-ingestion (tests/emul/normalize_emul.cpp) in the emulation library that tests/emul/harness.py builds
-and loads."""
-import ctypes as C
-
+"""Ristretto255 generators in scaled representations, and the decoding of the device generators that
+the normalising ingestion writes."""
 import numpy as np
 
 P = 2 ** 255 - 19
@@ -54,44 +51,3 @@ def decode_device_gen(row):
     limbs = np.frombuffer(row.tobytes(), dtype="<u4").astype(object)
     return [sum(int(limbs[8 * c + i]) << (32 * i) for i in range(8)) for c in range(4)]
 
-
-def _lib():
-    from tests.emul import harness
-    return harness
-
-
-def commit(curve, columns, generators, ranges=1, normalize=1):
-    """emul_normalize_commit: b200_commit_device in `ranges` generator ranges."""
-    h = _lib()
-    desc, keep = h._desc(columns)
-    out = np.zeros((len(columns), h.SIZES[curve][2]), dtype=np.uint8)
-    h.lib().emul_normalize_commit(C.c_uint(curve), C.c_void_p(out.ctypes.data),
-                                  C.c_uint32(len(columns)), desc,
-                                  C.c_void_p(generators.ctypes.data), C.c_uint(ranges),
-                                  C.c_uint(normalize))
-    return out
-
-
-def commit_offsets(curve, columns, offsets, generators, ranges=1, normalize=1):
-    """emul_normalize_commit_offsets: b200_commit_device_with_offsets in `ranges` ranges."""
-    h = _lib()
-    desc, keep = h._desc(columns)
-    out = np.zeros((len(columns), h.SIZES[curve][2]), dtype=np.uint8)
-    offs = np.ascontiguousarray(offsets, dtype=np.uint64)
-    h.lib().emul_normalize_commit_offsets(C.c_uint(curve), C.c_void_p(out.ctypes.data),
-                                          C.c_uint32(len(columns)), desc,
-                                          C.c_void_p(generators.ctypes.data),
-                                          C.c_void_p(offs.ctypes.data), C.c_uint(ranges),
-                                          C.c_uint(normalize))
-    return out
-
-
-def ingest(generators, normalize=1):
-    """(device generators [n, 128] bytes, Z = 0 flag) as the ingestion writes them."""
-    h = _lib()
-    gens = np.ascontiguousarray(generators)
-    out = np.zeros((gens.shape[0], 128), dtype=np.uint8)
-    h.lib().emul_ingest_generators.restype = C.c_uint
-    flag = h.lib().emul_ingest_generators(C.c_void_p(gens.ctypes.data), C.c_uint64(gens.shape[0]),
-                                          C.c_void_p(out.ctypes.data), C.c_uint(normalize))
-    return out, int(flag)

@@ -3,7 +3,6 @@
 input generators, and the digest rule (SHA-256 of the table bytes after the u32 window-width header;
 ristretto255 tables are canonicalised first, because the reference's radix-2^51 limbs are not
 guaranteed canonical, so they compare by value)."""
-import ctypes as C
 import hashlib
 
 import numpy as np
@@ -12,7 +11,6 @@ from tests import common
 
 P25519 = (1 << 255) - 19
 MASK51 = (1 << 51) - 1
-COMPACT_BYTES = {0: 120, 1: 96, 2: 64, 3: 64}  # c21t / cg1t / cn1t / cgkt::compact_element
 # name -> (n, window width, edited generators)
 CASES = {"n37_w8": (37, 8, False), "n24_w6_edited": (24, 6, True), "n16_w16": (16, 16, False)}
 
@@ -86,15 +84,3 @@ def case_generators(port, curve, name):
     gens_p = np.array(gens_p, copy=True)
     return edit_generators(curve, gens_p) if edited else gens_p
 
-
-def emulated_table(emul, curve_id, generators_p, window_width, chunk_groups=0):
-    """The partition table (no header) of projective ABI generators, through the product's kernel
-    bodies run as serial host loops (tests/emul/ptable_emul.cpp), `chunk_groups` groups per chunk
-    (0 = one chunk). emul: the tests/emul/harness module."""
-    generators_p = np.ascontiguousarray(generators_p, dtype=np.uint8)
-    n = generators_p.shape[0]
-    out = np.zeros(-(-n // window_width) * (COMPACT_BYTES[curve_id] << window_width), dtype=np.uint8)
-    emul.lib().emul_partition_table(C.c_uint(curve_id), C.c_void_p(out.ctypes.data),
-                                    C.c_void_p(generators_p.ctypes.data), C.c_uint64(n),
-                                    C.c_uint(window_width), C.c_uint64(chunk_groups))
-    return out

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from tests import common
-from tests import commit_offsets_emul as eo
+from tests.emul import harness
 
 N = 120
 # ragged unsigned / signed columns, one of them empty
@@ -46,9 +46,8 @@ def columns(seed, shapes=SHAPES, n=N):
 
 @pytest.fixture(autouse=True)
 def default_options():
-    eo.configure()
-    yield
-    eo.configure()
+    with harness.options():
+        yield
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
@@ -57,7 +56,7 @@ def test_explicit_generators(port, curve, pattern):
     cols = columns(10 * curve + len(pattern))
     offsets = offset_patterns(lengths())[pattern]
     gens, _ = common.generators_for(port, curve, max(o + n for o, n in zip(offsets, lengths())))
-    got = eo.commit_offsets(curve, cols, offsets, gens)
+    got = harness.commit_offsets(curve, cols, offsets, gens)
     assert common.same(curve, got, oracle(port, curve, cols, offsets, gens))
 
 
@@ -65,7 +64,7 @@ def test_explicit_generators(port, curve, pattern):
 def test_builtin_generators(port, pattern):
     cols = columns(len(pattern))
     offsets = FAR if pattern == "far" else offset_patterns(lengths())[pattern]
-    got = eo.commit_offsets(0, cols, offsets)
+    got = harness.commit_offsets(0, cols, offsets)
     assert np.array_equal(got, oracle(port, 0, cols, offsets, None))
 
 
@@ -73,15 +72,15 @@ def test_builtin_generators(port, pattern):
 def test_no_offsets_and_equal_offsets_match_the_existing_call(emul, port, curve):
     cols = columns(50 + curve)
     gens, _ = common.generators_for(port, curve, N + 40)
-    assert np.array_equal(eo.commit_offsets(curve, cols, None, gens), emul.commit(curve, cols, gens))
-    assert np.array_equal(eo.commit_offsets(curve, cols, [0] * len(cols), gens),
+    assert np.array_equal(emul.commit_offsets(curve, cols, None, gens), emul.commit(curve, cols, gens))
+    assert np.array_equal(emul.commit_offsets(curve, cols, [0] * len(cols), gens),
                           emul.commit(curve, cols, gens))
-    assert np.array_equal(eo.commit_offsets(curve, cols, [40] * len(cols), gens),
+    assert np.array_equal(emul.commit_offsets(curve, cols, [40] * len(cols), gens),
                           emul.commit(curve, cols, gens[40:]))
     if curve == 0:
-        assert np.array_equal(eo.commit_offsets(0, cols, None), emul.commit(0, cols))
+        assert np.array_equal(emul.commit_offsets(0, cols, None), emul.commit(0, cols))
         for off in (0, 17, 1 << 33):
-            assert np.array_equal(eo.commit_offsets(0, cols, [off] * len(cols)),
+            assert np.array_equal(emul.commit_offsets(0, cols, [off] * len(cols)),
                                   emul.commit(0, cols, None, off)), off
 
 
@@ -89,7 +88,7 @@ def test_only_empty_columns(port):
     cols = [(np.zeros((0, 4), np.uint8), 0), (np.zeros((0, 16), np.uint8), 1)]
     for curve in range(4):
         gens, _ = common.generators_for(port, curve, 1)
-        got = eo.commit_offsets(curve, cols, [5, 1 << 40], gens if curve else None)
+        got = harness.commit_offsets(curve, cols, [5, 1 << 40], gens if curve else None)
         assert common.same(curve, got, oracle(port, curve, cols, [5, 1 << 40], gens if curve else None))
 
 
@@ -98,13 +97,13 @@ def test_only_empty_columns(port):
 def test_upload_pieces(port, curve, ranges):
     """Each generator range ingests (or generates) only the packed positions its rows use."""
     cols = columns(70 + ranges)
-    eo.configure(ranges=ranges)
+    harness.configure(ranges=ranges)
     for pattern, offsets in offset_patterns(lengths()).items():
         gens, _ = common.generators_for(port, curve, max(o + n for o, n in zip(offsets, lengths())))
-        got = eo.commit_offsets(curve, cols, offsets, gens)
+        got = harness.commit_offsets(curve, cols, offsets, gens)
         assert common.same(curve, got, oracle(port, curve, cols, offsets, gens)), pattern
     if curve == 0:
-        got = eo.commit_offsets(0, cols, FAR)
+        got = harness.commit_offsets(0, cols, FAR)
         assert np.array_equal(got, oracle(port, 0, cols, FAR, None))
 
 
@@ -115,11 +114,11 @@ def test_sort_passes_and_column_groups(port, curve):
     gens, _ = common.generators_for(port, curve, 300)
     want = oracle(port, curve, cols, offsets, gens)
     for range_entries, group_entries in ((300, 0), (0, 400), (500, 700)):
-        eo.configure(range_entries=range_entries, group_entries=group_entries)
-        got = eo.commit_offsets(curve, cols, offsets, gens)
+        harness.configure(range_entries=range_entries, group_entries=group_entries)
+        got = harness.commit_offsets(curve, cols, offsets, gens)
         assert common.same(curve, got, want), (range_entries, group_entries)
         if curve == 0:
-            got = eo.commit_offsets(0, cols, FAR)
+            got = harness.commit_offsets(0, cols, FAR)
             assert np.array_equal(got, oracle(port, 0, cols, FAR, None)), (range_entries, group_entries)
 
 
@@ -132,21 +131,21 @@ def test_builtin_table(port, policy):
                     [0, 300, 60, 15, 100, 45],  # straddling (300 + 120 > 400)
                     [400, 500, 1000, 401, 2000, 450],  # beyond
                     FAR):
-        eo.configure(table_policy=policy, num_builtin=400, window_bits=8)
-        assert np.array_equal(eo.commit_offsets(0, cols, offsets),
+        harness.configure(table_policy=policy, num_builtin=400, builtin_window=8)
+        assert np.array_equal(harness.commit_offsets(0, cols, offsets),
                               oracle(port, 0, cols, offsets, None)), offsets
-        eo.configure(ranges=3, table_policy=policy, num_builtin=400, window_bits=8)
-        assert np.array_equal(eo.commit_offsets(0, cols, offsets),
+        harness.configure(ranges=3, table_policy=policy, num_builtin=400, builtin_window=8)
+        assert np.array_equal(harness.commit_offsets(0, cols, offsets),
                               oracle(port, 0, cols, offsets, None)), offsets
 
 
 @pytest.mark.parametrize("curve", [1, 2, 3])
 @pytest.mark.parametrize("levels", [0, 1, 3])
 def test_pair_levels(port, curve, levels):
-    eo.configure(pair_levels=levels)
+    harness.configure(pair_levels=levels)
     cols = columns(100 + curve, [(0, 32, 0), (-20, 16, 1), (0, 1, 0), (-N, 8, 0)])
     lens = lengths([(0, 32, 0), (-20, 16, 1), (0, 1, 0), (-N, 8, 0)])
     for offsets in ([0, 30, 60, 15], [0, 500, 200, 900]):
         gens, _ = common.generators_for(port, curve, max(o + n for o, n in zip(offsets, lens)) + 1)
-        got = eo.commit_offsets(curve, cols, offsets, gens)
+        got = harness.commit_offsets(curve, cols, offsets, gens)
         assert common.same(curve, got, oracle(port, curve, cols, offsets, gens)), offsets

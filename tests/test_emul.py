@@ -15,9 +15,8 @@ def test_production_multiply_schedules_match_reference_schedules(emul):
 
 
 def test_binary_euclid_inversion_matches_fermat(emul):
-    import ctypes as C
     for field_id in (1, 2, 3):
-        assert int(emul.lib().emul_check_invert(C.c_uint(field_id), C.c_uint(300), C.c_uint(field_id))) == 0
+        assert emul.check_invert(field_id, 300, field_id) == 0
 
 
 def test_golden_commitments(emul):
@@ -52,11 +51,8 @@ def test_every_window_width(emul, port, window_bits):
     n = 300
     gens, _ = common.generators_for(port, 0, n)
     cols = common.random_columns(rng, n, [(0, 32, 0), (-3, 4, 1), (0, 7, 0)])
-    try:
-        emul.set_tuning(window_bits=window_bits)
+    with emul.options(window_bits=window_bits):
         got = emul.commit(0, cols, gens)
-    finally:
-        emul.set_tuning()
     assert common.same(0, got, port.commit(0, cols, gens))
 
 
@@ -71,11 +67,8 @@ def test_cascade_chunk_shapes_and_skew(emul, port, chunks):
     two = np.zeros((n, 4), dtype=np.uint8)
     two[:, 0] = rng.integers(1, 3, n)
     cols = [(skew, 0), (two, 0)] + common.random_columns(rng, n, [(0, 32, 0)])
-    try:
-        emul.set_tuning(chunk1=chunks[0], chunkn=chunks[1])
+    with emul.options(chunk1=chunks[0], chunkn=chunks[1]):
         got = emul.commit(0, cols, gens)
-    finally:
-        emul.set_tuning()
     assert common.same(0, got, port.commit(0, cols, gens))
 
 
@@ -144,8 +137,7 @@ def test_identity_generators_in_pair_levels(emul, port, levels):
     """Identity generators as operands of the batch-affine pair levels (a column of ones pairs them
     with real points), and projective handle generators with Z = 0, with and without the table."""
     rng = np.random.default_rng(4)
-    try:
-        emul.set_pairs(levels, 0)
+    with emul.options(pair_levels=levels):
         for curve in (1, 2, 3):
             gens, gens_p = common.generators_for(port, curve, 20)
             gens, gens_p = gens.copy(), gens_p.copy()
@@ -159,12 +151,10 @@ def test_identity_generators_in_pair_levels(emul, port, levels):
             sc[:, 32] = 1
             want = port.normalize(curve, port.fixed_msm(curve, gens_p, 2, 20, sc, element_num_bytes=32))
             for table in (0, 10):
-                emul.set_table(table, 1 if table else 0)
+                emul.configure(pair_levels=levels, table_window=table,
+                               table_policy=1 if table else 0)
                 got = emul.fixed_msm(curve, gens_p, 2, 20, sc, element_num_bytes=32)
                 assert common.same(curve, port.normalize(curve, got), want), (curve, table)
-    finally:
-        emul.set_pairs(-1, 0)
-        emul.set_table(0, 0)
 
 
 @pytest.mark.parametrize("curve", [0, 2])
@@ -176,12 +166,9 @@ def test_generator_ranges_share_one_bucket_array(emul, port, curve, num_ranges):
     n = 500
     gens, _ = common.generators_for(port, curve, n)
     cols = common.random_columns(rng, n, [(0, 32, 0), (-300, 16, 1), (-499, 4, 0), (0, 1, 0)])
-    try:
-        emul.set_ranges(num_ranges)
+    with emul.options(ranges=num_ranges):
         got = emul.commit(curve, cols, gens)
         got_builtin = emul.commit(0, cols[:2], None, 5) if curve == 0 else None
-    finally:
-        emul.set_ranges(1)
     assert common.same(curve, got, port.commit(curve, cols, gens))
     if got_builtin is not None:
         assert common.same(0, got_builtin, port.commit(0, cols[:2], None, 5))
@@ -196,14 +183,9 @@ def test_column_groups_with_generator_ranges(emul, port):
     n = 400
     gens, _ = common.generators_for(port, 0, n)
     cols = common.random_columns(rng, n, [(0, 32, 0), (-100, 16, 1), (0, 8, 0), (-399, 32, 0), (0, 4, 0)])
-    try:
-        emul.set_ranges(3)
-        emul.set_group_entries(4000)
+    with emul.options(ranges=3, group_entries=4000):
         got = emul.commit(0, cols, gens)
         got_builtin = emul.commit(0, cols, None, 9)
-    finally:
-        emul.set_ranges(1)
-        emul.set_group_entries(0)
     assert common.same(0, got, port.commit(0, cols, gens))
     assert common.same(0, got_builtin, port.commit(0, cols, None, 9))
 
@@ -215,11 +197,8 @@ def test_long_columns_split_into_sort_passes(emul, port):
     n = 600
     gens, _ = common.generators_for(port, 2, n)
     cols = common.random_columns(rng, n, [(0, 32, 0), (-250, 8, 1)])
-    try:
-        emul.set_range_entries(3000)
+    with emul.options(range_entries=3000):
         got = emul.commit(2, cols, gens)
-    finally:
-        emul.set_range_entries(0)
     assert common.same(2, got, port.commit(2, cols, gens))
 
 
@@ -233,8 +212,7 @@ def test_fixed_base_table_mode(emul, port, curve, window_bits):
     rng = np.random.default_rng(40 + curve + window_bits)
     m = 400
     _, gens_p = common.generators_for(port, curve, m)
-    try:
-        emul.set_table(window_bits, 1)
+    with emul.options(table_window=window_bits, table_policy=1):
         sc = rng.integers(0, 256, (m, 2 * 32), dtype=np.uint8)
         a = emul.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
         b = port.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
@@ -245,12 +223,11 @@ def test_fixed_base_table_mode(emul, port, curve, window_bits):
         a = emul.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt, output_lengths=lens)
         b = port.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt, output_lengths=lens)
         assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b))
-        emul.set_table(window_bits, 0)  # cost model: short columns fall back to the variable-base run
+        # cost model: short columns fall back to the variable-base run
+        emul.configure(table_window=window_bits, table_policy=0)
         a = emul.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt)
         b = port.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt)
         assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b))
-    finally:
-        emul.set_table(0, 0)
 
 
 def test_builtin_generator_table(emul, port):
@@ -258,15 +235,10 @@ def test_builtin_generator_table(emul, port):
     generators inside, straddling and beyond the table."""
     rng = np.random.default_rng(77)
     cols = common.random_columns(rng, 300, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-299, 8, 0)])
-    try:
-        for c in (0, 12):
-            emul.set_builtin(400, c)
-            emul.set_table(0, 1 if c else 0)
+    for c in (0, 12):
+        with emul.options(num_builtin=400, builtin_window=c, table_policy=1 if c else 0):
             for off in (0, 37, 100, 250):
                 assert np.array_equal(emul.commit(0, cols, None, off), port.commit(0, cols, None, off))
-    finally:
-        emul.set_builtin(0, 0)
-        emul.set_table(0, 0)
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
@@ -292,11 +264,8 @@ def test_window_major_scatter_option(emul, port):
     n = 500
     gens, _ = common.generators_for(port, 0, n)
     cols = common.random_columns(rng, n, [(0, 32, 0), (-13, 16, 1), (0, 8, 1), (-499, 32, 0), (0, 1, 0)])
-    try:
-        emul.set_scatter_window_major(1)
+    with emul.options(scatter_window_major=1):
         assert common.same(0, emul.commit(0, cols, gens), port.commit(0, cols, gens))
-    finally:
-        emul.set_scatter_window_major(0)
 
 
 @pytest.mark.parametrize("curve", [1, 2, 3])
@@ -314,19 +283,12 @@ def test_batch_affine_pair_levels(emul, port, curve):
     sg[::2], sg[1::2] = 1, 0xFF  # +1 / -1 alternating: P + (-P) on the duplicated generators
     cols += [(ones, 0), (sg, 1)]
     want = port.commit(curve, cols, gens)
-    try:
-        for c, levels, batch in ((4, 1, 4), (4, 3, 5), (6, 2, 32), (3, 5, 0), (2, 6, 64), (0, 6, 1)):
-            emul.set_tuning(window_bits=c)
-            emul.set_pairs(levels, batch)
+    for c, levels, batch in ((4, 1, 4), (4, 3, 5), (6, 2, 32), (3, 5, 0), (2, 6, 64), (0, 6, 1)):
+        with emul.options(window_bits=c, pair_levels=levels, pair_batch=batch):
             assert common.same(curve, emul.commit(curve, cols, gens), want), (c, levels, batch)
-        emul.set_ranges(3)  # later ranges: scratch buckets + merge with padded layouts
-        emul.set_tuning(window_bits=4)
-        emul.set_pairs(2, 8)
+    # later ranges: scratch buckets + merge with padded layouts
+    with emul.options(ranges=3, window_bits=4, pair_levels=2, pair_batch=8):
         assert common.same(curve, emul.commit(curve, cols, gens), want)
-    finally:
-        emul.set_ranges(1)
-        emul.set_tuning()
-        emul.set_pairs(-1, 0)
 
 
 @pytest.mark.parametrize("curve", [1, 2, 3])
@@ -339,12 +301,9 @@ def test_degenerate_pair_level_buckets(emul, port, curve):
     for j, m in equal:
         assert common.same(curve, want[j:j + 1],
                            port.commit(curve, [(np.array([[m]], dtype=np.uint8), 0)], gens[:1])), m
-    try:
-        for levels in (-1, 1, 2, 3, 4, 5, 6):
-            emul.set_pairs(levels, 0)
+    for levels in (-1, 1, 2, 3, 4, 5, 6):
+        with emul.options(pair_levels=levels):
             assert common.same(curve, emul.commit(curve, cols, gens), want), levels
-    finally:
-        emul.set_pairs(-1, 0)
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
@@ -356,15 +315,10 @@ def test_fixed_base_table_cross_window_collisions(emul, port, curve, window_bits
     gens_p, sc = common.cross_window_handle(port, curve, window_bits)
     m = gens_p.shape[0]
     want = port.normalize(curve, port.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32))
-    try:
-        emul.set_table(window_bits, 1)
-        for levels in (-1, 1, 2, 3):
-            emul.set_pairs(levels, 0)
+    for levels in (-1, 1, 2, 3):
+        with emul.options(table_window=window_bits, table_policy=1, pair_levels=levels):
             got = emul.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
             assert common.same(curve, port.normalize(curve, got), want), levels
-    finally:
-        emul.set_table(0, 0)
-        emul.set_pairs(-1, 0)
 
 
 @pytest.mark.parametrize("curve", [1, 2, 3])
@@ -388,8 +342,5 @@ def test_edited_synthetic_generators_keep_the_closed_form(emul, port, curve):
     ed.identity(slice(5, n, 31))
     want = port.commit(curve, [(s, 0)], gens)
     assert common.same(curve, common.closed_form_commitment(port, curve, s, k=ed.k), want)
-    try:
-        emul.set_pairs(2, 0)
+    with emul.options(pair_levels=2):
         assert common.same(curve, emul.commit(curve, [(s, 0)], gens), want)
-    finally:
-        emul.set_pairs(-1, 0)

@@ -9,6 +9,7 @@ import pytest
 
 from tests import common
 from tests import normalize_emul as ne
+from tests.emul import harness
 
 N = 300
 SHAPES = [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-250, 8, 0)]
@@ -21,16 +22,17 @@ def _gens(port, n, seed, **kw):
 
 def test_ingestion_writes_unit_z(port):
     gens = _gens(port, 50, 1, **SPECIAL)
-    dev, flag = ne.ingest(gens)
+    dev, flag = harness.ingest_generators(gens)
     assert flag == 0
     for row in dev:
         ypx, ymx, z2, t2d = ne.decode_device_gen(row)
         assert z2 == 2 and max(ypx, ymx, t2d) < ne.P  # Z = 1, every field canonical
     # Z = 0 anywhere: the generators are written exactly as without the normalisation
     bad = _gens(port, 50, 2, zero_z=(17,), **SPECIAL)
-    dev, flag = ne.ingest(bad)
+    dev, flag = harness.ingest_generators(bad)
     assert flag == 1
-    assert np.array_equal(dev, ne.ingest(bad, normalize=0)[0])
+    with harness.options(normalize=0):
+        assert np.array_equal(dev, harness.ingest_generators(bad)[0])
 
 
 @pytest.mark.parametrize("ranges", [1, 3])
@@ -40,8 +42,10 @@ def test_device_call(port, ranges):
     # the oracle sees the same points in their plain representation
     plain = ne.scaled_generators(port.ristretto_generators(N), 0, scale=False, **SPECIAL)
     want = port.commit(0, cols, plain)
-    on = ne.commit(0, cols, gens, ranges, normalize=1)
-    off = ne.commit(0, cols, gens, ranges, normalize=0)
+    with harness.options(ranges=ranges, normalize=1):
+        on = harness.commit(0, cols, gens)
+    with harness.options(ranges=ranges, normalize=0):
+        off = harness.commit(0, cols, gens)
     assert np.array_equal(on, want)
     assert np.array_equal(off, want)
 
@@ -51,8 +55,10 @@ def test_device_call(port, ranges):
 def test_zero_z_keeps_todays_bytes(port, ranges, zero_at):
     cols = common.random_columns(np.random.default_rng(30 + ranges), N, SHAPES)
     gens = _gens(port, N, 40 + zero_at, zero_z=(zero_at,), **SPECIAL)
-    on = ne.commit(0, cols, gens, ranges, normalize=1)
-    off = ne.commit(0, cols, gens, ranges, normalize=0)
+    with harness.options(ranges=ranges, normalize=1):
+        on = harness.commit(0, cols, gens)
+    with harness.options(ranges=ranges, normalize=0):
+        off = harness.commit(0, cols, gens)
     assert np.array_equal(on, off)
 
 
@@ -62,13 +68,19 @@ def test_offsets_call(port, ranges):
     offsets = [0, 400, 120, 37]
     total = max(o + N for o in offsets)
     gens = _gens(port, total, 60 + ranges, **SPECIAL)
-    want = ne.commit_offsets(0, cols, offsets, gens, ranges, normalize=0)
-    got = ne.commit_offsets(0, cols, offsets, gens, ranges, normalize=1)
+    with harness.options(ranges=ranges, normalize=0):
+        want = harness.commit_offsets(0, cols, offsets, gens)
+    with harness.options(ranges=ranges, normalize=1):
+        got = harness.commit_offsets(0, cols, offsets, gens)
     assert np.array_equal(got, want)
     # every column equals the device call over its own generators
     for j, off in enumerate(offsets):
-        one = ne.commit(0, [cols[j]], np.ascontiguousarray(gens[off:off + N]), normalize=0)
+        with harness.options(normalize=0):
+            one = harness.commit(0, [cols[j]], np.ascontiguousarray(gens[off:off + N]))
         assert np.array_equal(got[j:j + 1], one), j
     bad = _gens(port, total, 70 + ranges, zero_z=(405,), **SPECIAL)
-    assert np.array_equal(ne.commit_offsets(0, cols, offsets, bad, ranges, normalize=1),
-                          ne.commit_offsets(0, cols, offsets, bad, ranges, normalize=0))
+    with harness.options(ranges=ranges, normalize=1):
+        bad_on = harness.commit_offsets(0, cols, offsets, bad)
+    with harness.options(ranges=ranges, normalize=0):
+        bad_off = harness.commit_offsets(0, cols, offsets, bad)
+    assert np.array_equal(bad_on, bad_off)

@@ -17,10 +17,10 @@ def test_reference_w3_file_is_reproduced(emul, curve):
     g7 = np.load(os.path.join(GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
     ref = np.fromfile(os.path.join(GOLDEN, f"ref_table_curve{curve}_w3.bin"), dtype=np.uint8)
     assert int(ref[:4].view("<u4")[0]) == 3
-    got = pt.emulated_table(emul, curve, g7, 3)
+    got = emul.partition_table(curve, g7, 3)
     want = pt.canonicalise_ristretto_table(ref[4:]) if curve == 0 else ref[4:]
     assert np.array_equal(got, want)
-    assert np.array_equal(pt.emulated_table(emul, curve, g7, 3, chunk_groups=1), got)
+    assert np.array_equal(emul.partition_table(curve, g7, 3, chunk_groups=1), got)
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
@@ -29,12 +29,12 @@ def test_fixture_digests(emul, curve, case):
     z = np.load(os.path.join(GOLDEN, f"ptable_curve{curve}.npz"))
     gens = z[f"gens_{case}"]
     _, w, _ = pt.CASES[case]
-    got = pt.emulated_table(emul, curve, gens, w)
+    got = emul.partition_table(curve, gens, w)
     # the device writes canonical limbs: its raw bytes already carry the canonicalised digest
     assert pt.table_digest(curve, got) == str(z[f"sha_{case}"])
     assert pt.sha256(got) == str(z[f"sha_{case}"])
     if w < 16:
-        assert np.array_equal(pt.emulated_table(emul, curve, gens, w, chunk_groups=3), got)
+        assert np.array_equal(emul.partition_table(curve, gens, w, chunk_groups=3), got)
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
@@ -48,7 +48,7 @@ def test_generators_read_back(emul, port, curve, tmp_path):
         path = str(tmp_path / f"{case}.bin")
         with open(path, "wb") as f:
             f.write(np.uint32(w).tobytes())
-            f.write(pt.emulated_table(emul, curve, gens, w).tobytes())
+            f.write(emul.partition_table(curve, gens, w).tobytes())
         back = emul.generators_from_reference_table(curve, path)
         n = gens.shape[0]
         assert back.shape[0] == -(-n // w) * w
