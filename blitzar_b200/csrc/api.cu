@@ -154,6 +154,11 @@ void require_init(const char* fn) {
   }
   B200_CUDA(cudaSetDevice(g_state.device));
 }
+// one entry point's hold on the library: the call lock, then the sxt_init check
+struct Entry {
+  std::lock_guard<std::mutex> lock{g_mutex};
+  explicit Entry(const char* fn) { require_init(fn); }
+};
 
 
 // Host-to-device upload of PAGEABLE caller memory. A plain cudaMemcpyAsync from pageable memory is
@@ -284,19 +289,6 @@ private:
   }
 };
 
-// validates like cbindings/pedersen.cc:44-68 and returns the longest column
-uint64_t longest_column(const sxt_sequence_descriptor* d, uint32_t num) {
-  B200_REQUIRE(d != nullptr, "descriptors == nullptr");
-  uint64_t longest = 0;
-  for (uint32_t i = 0; i < num; ++i) {
-    B200_REQUIRE(d[i].n == 0 || d[i].data != nullptr, "descriptor.n > 0 with data == nullptr");
-    B200_REQUIRE(d[i].element_nbytes != 0 && d[i].element_nbytes <= 32,
-                 "descriptor.element_nbytes must be in 1..32");
-    longest = longest < d[i].n ? d[i].n : longest;
-  }
-  return longest;
-}
-
 // Host-pointer commitments. The generator range is split into pieces; the copy stream uploads piece
 // after piece (scalars rows + generators) while the compute stream sorts and accumulates the
 // previous one into the shared bucket array, so most of the PCIe time hides behind the kernels.
@@ -336,13 +328,14 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
   const CurveVTable& V = curve_vtable(curve_id);
   StageRange nvtx("commit (host buffers)");
   cudaStream_t s = st.stream, sc = st.copy_stream;
-  uint64_t n = longest_column(d, num);
+  const uint64_t n = check_descriptors(d, num);
   size_t total_scalar_bytes = 0;
   for (uint32_t i = 0; i < num; ++i)
     total_scalar_bytes += (size_t)d[i].n * d[i].element_nbytes + 32;
-  // per-column offsets: the device holds only the generators the columns use, in the packed order
-  std::unique_ptr<GenLayout> layout(offsets ? new GenLayout(d, num, offsets) : nullptr);
-  DevBuf<unsigned char> raw_gens(generators ? (layout ? layout->total : n) * V.abi_gen_bytes : 1, s);
+  // the device holds only the generators the columns use, in the layout's packed order (without
+  // offsets: generators [0, n) where they are)
+  const GenLayout layout(d, num, offsets);
+  DevBuf<unsigned char> raw_gens(generators ? layout.total * V.abi_gen_bytes : 1, s);
   DevBuf<unsigned char> scal(total_scalar_bytes, s);
   DevBuf<unsigned char> out((size_t)num * V.abi_commit_bytes, s);
   std::vector<sxt_sequence_descriptor> dd(d, d + num);
@@ -398,16 +391,11 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
                              d[i].data + lo * d[i].element_nbytes,
                              (hi - lo) * d[i].element_nbytes, sc);
     }
-    if (generators && layout) {
-      for (const GenLayout::Piece& p : layout->needed(b, e))
+    if (generators)
+      for (const GenLayout::Piece& p : layout.needed(b, e))
         HostStager::get().copy(raw_gens.p + p.pos * V.abi_gen_bytes,
                                static_cast<const unsigned char*>(generators) + p.src * V.abi_gen_bytes,
                                p.count * V.abi_gen_bytes, sc);
-    } else if (generators) {
-      HostStager::get().copy(raw_gens.p + b * V.abi_gen_bytes,
-                             static_cast<const unsigned char*>(generators) + b * V.abi_gen_bytes,
-                             (e - b) * V.abi_gen_bytes, sc);
-    }
     B200_CUDA(cudaEventRecord(st.range_events[r], sc));
     mark(sc);
   };
@@ -417,7 +405,7 @@ void commit_on(const State& st, unsigned curve_id, void* commitments, uint32_t n
   RangeWaitState w{n, num_ranges, skew, &st, 0, upload};
   EngineCtx cx = ctx_of(st);
   cx.opt.range_skew = skew;
-  if (layout)
+  if (offsets)
     V.commit_device_offsets(cx, out_partials_dev ? nullptr : out.p, out_partials_dev, num, dd.data(),
                             generators ? raw_gens.p : nullptr, offsets, true, num_ranges,
                             &wait_for_range, &w);
@@ -547,15 +535,44 @@ template <class F> void on_devices(size_t parts, F f) {
     g_workers[p - 1]->wait();
   B200_CUDA(cudaSetDevice(g_state.device));
 }
-// this shard's `count` partial points -> slot `part` of the primary device's gather buffer
-void send_partials(const State& st, size_t part, const void* partials_dev, size_t bytes,
-                   void* gather_base) {
-  unsigned char* dst = static_cast<unsigned char*>(gather_base) + part * bytes;
-  if (part == 0)
-    B200_CUDA(cudaMemcpyAsync(dst, partials_dev, bytes, cudaMemcpyDeviceToDevice, st.stream));
-  else
-    B200_CUDA(cudaMemcpyPeerAsync(dst, g_state.device, partials_dev, st.device, bytes, st.stream));
-  B200_CUDA(cudaStreamSynchronize(st.stream));
+// run(st, p, partials_dev) for p = 0 .. parts-1 on the devices (on_devices): each writes `count`
+// partial points into partials_dev on st's device. They are gathered in g_gather on the primary
+// device and summed there into `sum` (count points on the primary device).
+template <class F>
+void sum_over_devices(const CurveVTable& V, size_t parts, uint32_t count, void* sum, F run) {
+  const size_t bytes = (size_t)count * V.point_bytes;
+  unsigned char* gather = static_cast<unsigned char*>(g_gather.ensure(parts * bytes));
+  on_devices(parts, [&](size_t p) {
+    const State& st = state_of(p);
+    DevBuf<unsigned char> partials(bytes, st.stream);
+    run(st, p, partials.p);
+    if (p == 0)
+      B200_CUDA(cudaMemcpyAsync(gather, partials.p, bytes, cudaMemcpyDeviceToDevice, st.stream));
+    else
+      B200_CUDA(cudaMemcpyPeerAsync(gather + p * bytes, g_state.device, partials.p, st.device, bytes,
+                                    st.stream));
+    B200_CUDA(cudaStreamSynchronize(st.stream));
+  });
+  V.sum_parts(ctx(), gather, (uint32_t)parts, count, sum);
+}
+// `count` accumulator points on the primary device -> commitments (commit) or projective ABI
+// structs in host memory
+void store_to_host(const CurveVTable& V, const void* pts, uint32_t count, bool commit, void* host) {
+  cudaStream_t s = g_state.stream;
+  const size_t bytes = (size_t)count * (commit ? V.abi_commit_bytes : V.abi_proj_bytes);
+  DevBuf<unsigned char> out(bytes, s);
+  V.store(ctx(), pts, out.p, count, commit);
+  copy_d2h(host, out.p, bytes, s);
+  stream_sync(s);
+}
+// the sums of num_parts x count partial points (device, part-major) -> count commitments (commit)
+// or projective ABI structs in device memory
+void combine_partials(unsigned curve_id, void* out_dev, const void* partials, uint32_t num_parts,
+                      uint32_t count, bool commit) {
+  const CurveVTable& V = curve_vtable(curve_id);
+  DevBuf<unsigned char> sum((size_t)count * V.point_bytes, g_state.stream);
+  V.sum_parts(ctx(), partials, num_parts, count, sum.p);
+  V.store(ctx(), sum.p, out_dev, count, commit);
 }
 
 void commit_host(unsigned curve_id, void* commitments, uint32_t num,
@@ -564,10 +581,9 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
                  const uint64_t* offsets = nullptr) {
   if (num == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init(fn);
+  const Entry entry(fn);
   B200_REQUIRE(commitments != nullptr || out_partials_dev != nullptr, "commitments == nullptr");
-  const uint64_t n = longest_column(d, num);  // validates the descriptors before any thread starts
+  const uint64_t n = check_descriptors(d, num);  // validates the descriptors before any thread starts
   if (curve_id != SXT_CURVE_RISTRETTO255)
     B200_REQUIRE(generators != nullptr, "generators == nullptr");
   if (offsets)
@@ -610,11 +626,8 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
               offsets);
     return;
   }
-  const size_t pbytes = (size_t)num * V.point_bytes;
-  void* gather = g_gather.ensure(parts * pbytes);
-  on_devices(parts, [&, curve_id, num, d, generators, offset_generators, n, parts, pbytes,
-                     gather](size_t p) {
-    State& st = state_of(p);
+  DevBuf<unsigned char> sum((size_t)num * V.point_bytes, g_state.stream);
+  sum_over_devices(V, parts, num, sum.p, [&](const State& st, size_t p, void* partials) {
     const uint64_t lo = n * p / parts, hi = n * (p + 1) / parts;
     std::vector<sxt_sequence_descriptor> dd(d, d + num);
     std::vector<uint64_t> part_offsets(offsets ? num : 0);  // each column's slice starts at row b
@@ -627,21 +640,13 @@ void commit_host(unsigned curve_id, void* commitments, uint32_t num,
         part_offsets[j] = offsets[j] + b;
     }
     const unsigned char* g = static_cast<const unsigned char*>(generators);
-    DevBuf<unsigned char> part(pbytes, st.stream);
     if (offsets)
-      commit_on(st, curve_id, nullptr, num, dd.data(), g, 0, part.p, part_offsets.data());
+      commit_on(st, curve_id, nullptr, num, dd.data(), g, 0, partials, part_offsets.data());
     else
       commit_on(st, curve_id, nullptr, num, dd.data(), g ? g + lo * V.abi_gen_bytes : nullptr,
-                offset_generators + lo, part.p);
-    send_partials(st, p, part.p, pbytes, gather);
+                offset_generators + lo, partials);
   });
-  cudaStream_t s = g_state.stream;
-  DevBuf<unsigned char> sum(pbytes, s);
-  DevBuf<unsigned char> out((size_t)num * stride, s);
-  V.sum_parts(ctx(), gather, (uint32_t)parts, num, sum.p);
-  V.store(ctx(), sum.p, out.p, num, true);
-  copy_d2h(commitments, out.p, (size_t)num * stride, s);
-  stream_sync(s);
+  store_to_host(V, sum.p, num, true, commitments);
 }
 
 // sxt_multiexp_handle: one shard per device (BLITZAR_B200_DEVICES=k splits the generator range at
@@ -651,6 +656,10 @@ struct HandleSet {
   std::vector<Handle*> shards;
   std::vector<unsigned> first;  // first generator of every shard
 };
+HandleSet* handle_of(const sxt_multiexp_handle* handle) {
+  B200_REQUIRE(handle != nullptr, "null handle");
+  return reinterpret_cast<HandleSet*>(const_cast<sxt_multiexp_handle*>(handle));
+}
 
 // One shard on st's device (the calling thread's current device). generators: n projective ABI
 // structs (host memory, or device_resident: already in HBM), or — compact_window != 0 — the table
@@ -705,17 +714,21 @@ uint64_t partition_chunk_groups(const CurveVTable& V, unsigned w) {
     bytes = std::strtoull(env, nullptr, 10);
   return std::max<uint64_t>(1, bytes / ((uint64_t)V.abi_compact_bytes << w));
 }
+// frees shard h's partition table, once the work queued on st's device that may read it is done
+void drop_partition_table(const State& st, Handle* h) {
+  stream_sync(st.stream);
+  B200_CUDA(cudaFree(h->ptable));
+  h->ptable = nullptr;
+  h->ptable_w = 0;
+  h->ptable_groups = 0;
+}
 // Replaces shard h's partition table (Handle::ptable) with one of width w, built on st's device in
 // chunks of whole groups. The table may take at most 40 % of the free HBM, as the fixed-base tables
 // do (choose_table_window); false, and no table, when it does not fit.
 bool shard_add_partition_table(const State& st, Handle* h, unsigned w) {
   const CurveVTable& V = curve_vtable(h->curve_id);
   cudaStream_t s = st.stream;
-  stream_sync(s);
-  B200_CUDA(cudaFree(h->ptable));
-  h->ptable = nullptr;
-  h->ptable_w = 0;
-  h->ptable_groups = 0;
+  drop_partition_table(st, h);
   const uint64_t groups = ((uint64_t)h->n + w - 1) / w;
   if (groups == 0)
     return false;
@@ -749,21 +762,14 @@ unsigned handle_add_partition_table(HandleSet* hs, unsigned window_width) {
   });
   if (std::find(ok.begin(), ok.end(), 0) == ok.end())
     return w;
-  on_devices(hs->shards.size(), [hs](size_t p) {
-    Handle* h = hs->shards[p];
-    stream_sync(state_of(p).stream);
-    B200_CUDA(cudaFree(h->ptable));
-    h->ptable = nullptr;
-    h->ptable_w = 0;
-    h->ptable_groups = 0;
-  });
+  on_devices(hs->shards.size(),
+             [hs](size_t p) { drop_partition_table(state_of(p), hs->shards[p]); });
   B200_LOG(1, "partition table of width %u does not fit in 40 %% of the free HBM", w);
   return 0;
 }
 
 HandleSet* handle_new(unsigned curve_id, const void* generators, unsigned n,
-                      bool device_resident = false, unsigned compact_window = 0,
-                      size_t compact_bytes = 0) {
+                      bool device_resident = false, unsigned compact_window = 0) {
   const CurveVTable& V = curve_vtable(curve_id);
   HandleSet* hs = new HandleSet;
   hs->curve_id = curve_id;
@@ -788,7 +794,6 @@ HandleSet* handle_new(unsigned curve_id, const void* generators, unsigned n,
     hs->shards[p] = shard_new(state_of(p), curve_id, g ? g + off : nullptr, cnt, device_resident,
                               compact_window, cbytes);
   });
-  (void)compact_bytes;
   // lets an unmodified sxt_* consumer opt in to partition tables at the reference's default width
   if (const char* env = std::getenv("BLITZAR_B200_PARTITION_HANDLES"))
     if (std::atoi(env) == 1)
@@ -836,17 +841,13 @@ void fixed_host(void* res, const HandleSet* hs, int mode, unsigned element_num_b
                 unsigned n, const uint8_t* scalars, void* out_partials_dev = nullptr) {
   if (num_outputs == 0)
     return;
-  FixedCall c{mode, element_num_bytes, bit_table, lengths, num_outputs, n, 0};
-  uint64_t row_bits = 0;
-  for (unsigned j = 0; j < num_outputs; ++j) {
-    row_bits += mode == 0 ? 8ull * element_num_bytes : bit_table[j];
-    if (mode == 2) {
-      B200_REQUIRE(j == 0 || lengths[j] >= lengths[j - 1],
-                   "output lengths must be sorted in ascending order");
-      c.rows = j == 0 ? lengths[j] : (lengths[j] > c.rows ? lengths[j] : c.rows);
-    }
+  FixedCall c{mode, element_num_bytes, bit_table, lengths, num_outputs, n,
+              fixed_row_bytes(mode, element_num_bytes, bit_table, num_outputs)};
+  if (mode == 2) {
+    for (unsigned j = 1; j < num_outputs; ++j)
+      B200_REQUIRE(lengths[j] >= lengths[j - 1], "output lengths must be sorted in ascending order");
+    c.rows = lengths[num_outputs - 1];
   }
-  c.row_bytes = (row_bits + 7) / 8;
   B200_REQUIRE(c.rows <= hs->n, "more scalars than generators in the handle");
   B200_REQUIRE(c.row_bytes * c.rows == 0 || scalars != nullptr, "scalars == nullptr");
   const size_t parts = hs->shards.size();
@@ -855,26 +856,17 @@ void fixed_host(void* res, const HandleSet* hs, int mode, unsigned element_num_b
     return;
   }
   const CurveVTable& V = curve_vtable(hs->curve_id);
-  const size_t pbytes = (size_t)num_outputs * V.point_bytes;
-  void* gather = g_gather.ensure(parts * pbytes);
-  on_devices(parts, [&, hs, scalars, pbytes, gather](size_t p) {
-    State& st = state_of(p);
-    DevBuf<unsigned char> part(pbytes, st.stream);
-    fixed_on(st, nullptr, hs->shards[p], c, hs->first[p], scalars, part.p);
-    send_partials(st, p, part.p, pbytes, gather);
-  });
-  cudaStream_t s = g_state.stream;
-  if (out_partials_dev) {
-    V.sum_parts(ctx(), gather, (uint32_t)parts, num_outputs, out_partials_dev);
-    stream_sync(s);
+  auto shard = [&](const State& st, size_t p, void* partials) {
+    fixed_on(st, nullptr, hs->shards[p], c, hs->first[p], scalars, partials);
+  };
+  if (out_partials_dev) {  // the summed points, unstored
+    sum_over_devices(V, parts, num_outputs, out_partials_dev, shard);
+    stream_sync(g_state.stream);
     return;
   }
-  DevBuf<unsigned char> sum(pbytes, s);
-  DevBuf<unsigned char> out((size_t)num_outputs * V.abi_proj_bytes, s);
-  V.sum_parts(ctx(), gather, (uint32_t)parts, num_outputs, sum.p);
-  V.store(ctx(), sum.p, out.p, num_outputs, false);
-  copy_d2h(res, out.p, (size_t)num_outputs * V.abi_proj_bytes, s);
-  stream_sync(s);
+  DevBuf<unsigned char> sum((size_t)num_outputs * V.point_bytes, g_state.stream);
+  sum_over_devices(V, parts, num_outputs, sum.p, shard);
+  store_to_host(V, sum.p, num_outputs, false, res);
 }
 
 const uint32_t kHandleMagic = 0x44483242u;  // "B2HD"
@@ -977,8 +969,7 @@ void sxt_grumpkin_uncompressed_compute_pedersen_commitments_with_generators(
 
 int sxt_ristretto255_get_generators(struct sxt_ristretto255* generators, uint64_t num_generators,
                                     uint64_t offset_generators) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_ristretto255_get_generators");
+  const Entry entry("sxt_ristretto255_get_generators");
   if (num_generators == 0)
     return 0;
   if (generators == nullptr)
@@ -995,8 +986,7 @@ int sxt_ristretto255_get_generators(struct sxt_ristretto255* generators, uint64_
 }
 
 int sxt_curve25519_get_one_commit(struct sxt_ristretto255* one_commit, uint64_t n) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_curve25519_get_one_commit");
+  const Entry entry("sxt_curve25519_get_one_commit");
   B200_REQUIRE(one_commit != nullptr, "one_commit == nullptr");
   B200_REQUIRE(n < (1ull << 31), "n too large");
   const CurveVTable& V = kVTableEd25519;
@@ -1006,11 +996,8 @@ int sxt_curve25519_get_one_commit(struct sxt_ristretto255* one_commit, uint64_t 
   B200_CUDA(cudaMemsetAsync(ones.p, 1, n + 32, s));
   sxt_sequence_descriptor d{1, n, ones.p, 0};
   DevBuf<unsigned char> pt(V.point_bytes, s);
-  DevBuf<unsigned char> out(V.abi_proj_bytes, s);
   V.commit_device(ctx(), nullptr, pt.p, 1, &d, nullptr, 0, 1, nullptr, nullptr);
-  V.store(ctx(), pt.p, out.p, 1, false);
-  copy_d2h(one_commit, out.p, V.abi_proj_bytes, s);
-  stream_sync(s);
+  store_to_host(V, pt.p, 1, false, one_commit);
   return 0;
 }
 
@@ -1022,8 +1009,7 @@ void sxt_curve25519_prove_inner_product(struct sxt_ristretto255_compressed* l_ve
                                         uint64_t generators_offset,
                                         const struct sxt_curve25519_scalar* a_vector,
                                         const struct sxt_curve25519_scalar* b_vector) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_curve25519_prove_inner_product");
+  const Entry entry("sxt_curve25519_prove_inner_product");
   B200_REQUIRE(transcript != nullptr, "transcript must not be null");
   B200_REQUIRE(ap_value != nullptr, "ap_value must not be null");
   B200_REQUIRE(b_vector != nullptr && a_vector != nullptr, "a_vector / b_vector must not be null");
@@ -1044,8 +1030,7 @@ int sxt_curve25519_verify_inner_product(struct sxt_transcript* transcript, uint6
                                         const struct sxt_ristretto255_compressed* l_vector,
                                         const struct sxt_ristretto255_compressed* r_vector,
                                         const struct sxt_curve25519_scalar* ap_value) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_curve25519_verify_inner_product");
+  const Entry entry("sxt_curve25519_verify_inner_product");
   B200_REQUIRE(transcript != nullptr, "transcript must not be null");
   B200_REQUIRE(ap_value != nullptr && product != nullptr && a_commit != nullptr &&
                    b_vector != nullptr,
@@ -1067,8 +1052,7 @@ void sxt_prove_sumcheck(void*, void*, unsigned, const struct sumcheck_descriptor
 
 struct sxt_multiexp_handle* sxt_multiexp_handle_new(unsigned curve_id, const void* generators,
                                                     unsigned n) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_multiexp_handle_new");
+  const Entry entry("sxt_multiexp_handle_new");
   return reinterpret_cast<sxt_multiexp_handle*>(handle_new(curve_id, generators, n));
 }
 
@@ -1076,11 +1060,10 @@ void sxt_multiexp_handle_free(struct sxt_multiexp_handle* handle) {
   if (!handle)
     return;
   std::lock_guard<std::mutex> lock(g_mutex);
-  HandleSet* hs = reinterpret_cast<HandleSet*>(handle);
+  HandleSet* hs = handle_of(handle);
   on_devices(hs->shards.size(), [hs](size_t p) {
-    B200_CUDA(cudaStreamSynchronize(state_of(p).stream));
+    drop_partition_table(state_of(p), hs->shards[p]);
     B200_CUDA(cudaFree(hs->shards[p]->gens));
-    B200_CUDA(cudaFree(hs->shards[p]->ptable));
     delete hs->shards[p];
   });
   delete hs;
@@ -1092,10 +1075,9 @@ void sxt_multiexp_handle_free(struct sxt_multiexp_handle* handle) {
 // file also reads the reference's [u32 window_width][partition table] files (see there).
 void sxt_multiexp_handle_write_to_file(const struct sxt_multiexp_handle* handle,
                                        const char* filename) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_multiexp_handle_write_to_file");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h && filename, "null handle or filename");
+  const Entry entry("sxt_multiexp_handle_write_to_file");
+  const HandleSet* h = handle_of(handle);
+  B200_REQUIRE(filename != nullptr, "null filename");
   const CurveVTable& V = curve_vtable(h->curve_id);
   size_t bytes = (size_t)h->n * V.abi_proj_bytes;
   std::vector<unsigned char> host(bytes);
@@ -1118,8 +1100,7 @@ void sxt_multiexp_handle_write_to_file(const struct sxt_multiexp_handle* handle,
 
 struct sxt_multiexp_handle* sxt_multiexp_handle_new_from_file(unsigned curve_id,
                                                               const char* filename) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_multiexp_handle_new_from_file");
+  const Entry entry("sxt_multiexp_handle_new_from_file");
   B200_REQUIRE(filename != nullptr, "null filename");
   FILE* f = std::fopen(filename, "rb");
   B200_REQUIRE(f != nullptr, "cannot open handle file");
@@ -1144,7 +1125,7 @@ struct sxt_multiexp_handle* sxt_multiexp_handle_new_from_file(unsigned curve_id,
     B200_REQUIRE(bytes == 0 || std::fread(host.data(), bytes, 1, f) == 1, "short handle file");
     std::fclose(f);
     return reinterpret_cast<sxt_multiexp_handle*>(
-        handle_new(curve_id, host.data(), (unsigned)(groups * w), false, w, bytes));
+        handle_new(curve_id, host.data(), (unsigned)(groups * w), false, w));
   }
   B200_REQUIRE(std::fread(hdr + 1, 3 * sizeof(uint32_t), 1, f) == 1, "short handle file");
   B200_REQUIRE(hdr[1] == 1u, "unsupported blitzar_b200 handle file version");
@@ -1159,30 +1140,21 @@ struct sxt_multiexp_handle* sxt_multiexp_handle_new_from_file(unsigned curve_id,
 void sxt_fixed_multiexponentiation(void* res, const struct sxt_multiexp_handle* handle,
                                    unsigned element_num_bytes, unsigned num_outputs, unsigned n,
                                    const uint8_t* scalars) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_fixed_multiexponentiation");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h != nullptr, "null handle");
-  fixed_host(res, h, 0, element_num_bytes, nullptr, nullptr, num_outputs, n, scalars);
+  const Entry entry("sxt_fixed_multiexponentiation");
+  fixed_host(res, handle_of(handle), 0, element_num_bytes, nullptr, nullptr, num_outputs, n, scalars);
 }
 void sxt_fixed_packed_multiexponentiation(void* res, const struct sxt_multiexp_handle* handle,
                                           const unsigned* output_bit_table, unsigned num_outputs,
                                           unsigned n, const uint8_t* scalars) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_fixed_packed_multiexponentiation");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h != nullptr, "null handle");
-  fixed_host(res, h, 1, 0, output_bit_table, nullptr, num_outputs, n, scalars);
+  const Entry entry("sxt_fixed_packed_multiexponentiation");
+  fixed_host(res, handle_of(handle), 1, 0, output_bit_table, nullptr, num_outputs, n, scalars);
 }
 void sxt_fixed_vlen_multiexponentiation(void* res, const struct sxt_multiexp_handle* handle,
                                         const unsigned* output_bit_table,
                                         const unsigned* output_lengths, unsigned num_outputs,
                                         const uint8_t* scalars) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("sxt_fixed_vlen_multiexponentiation");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h != nullptr, "null handle");
-  fixed_host(res, h, 2, 0, output_bit_table, output_lengths, num_outputs, 0, scalars);
+  const Entry entry("sxt_fixed_vlen_multiexponentiation");
+  fixed_host(res, handle_of(handle), 2, 0, output_bit_table, output_lengths, num_outputs, 0, scalars);
 }
 
 // =====================================================================================================
@@ -1196,8 +1168,7 @@ void b200_set_device(int device) {
 unsigned long long b200_launch_count(void) { return LaunchCounter::value(); }
 unsigned b200_point_bytes(unsigned curve_id) { return curve_vtable(curve_id).point_bytes; }
 void* b200_malloc(uint64_t bytes) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_malloc");
+  const Entry entry("b200_malloc");
   void* p = nullptr;
   B200_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
   return p;
@@ -1211,14 +1182,12 @@ void b200_free(void* p) {
   }
 }
 void b200_memcpy_h2d(void* d, const void* h, uint64_t bytes) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_memcpy_h2d");
+  const Entry entry("b200_memcpy_h2d");
   copy_h2d(d, h, bytes, g_state.stream);
   stream_sync(g_state.stream);
 }
 void b200_memcpy_d2h(void* h, const void* d, uint64_t bytes) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_memcpy_d2h");
+  const Entry entry("b200_memcpy_d2h");
   copy_d2h(h, d, bytes, g_state.stream);
   stream_sync(g_state.stream);
 }
@@ -1227,8 +1196,7 @@ void* b200_stream(void) {
   return (void*)g_state.stream;
 }
 void b200_synchronize(void) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_synchronize");
+  const Entry entry("b200_synchronize");
   stream_sync(g_state.stream);
 }
 void* b200_event_create(void) {
@@ -1254,8 +1222,7 @@ void b200_commit_device(unsigned curve_id, void* out_commitments, void* out_part
                         const void* generators, uint64_t offset_generators) {
   if (num_sequences == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_commit_device");
+  const Entry entry("b200_commit_device");
   curve_vtable(curve_id).commit_device(ctx(), out_commitments, out_partials, num_sequences,
                                        descriptors, generators, offset_generators, 1, nullptr,
                                        nullptr);
@@ -1273,8 +1240,7 @@ void b200_commit_device_with_offsets(unsigned curve_id, void* out_commitments, v
                                      const void* generators, const uint64_t* offsets) {
   if (num_sequences == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_commit_device_with_offsets");
+  const Entry entry("b200_commit_device_with_offsets");
   const CurveVTable& V = curve_vtable(curve_id);
   if (offsets)
     V.commit_device_offsets(ctx(), out_commitments, out_partials, num_sequences, descriptors,
@@ -1289,8 +1255,7 @@ void b200_commit_host_partials(unsigned curve_id, void* out_partials,
                                const void* generators, uint64_t offset_generators) {
   if (num_sequences == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_commit_host_partials");
+  const Entry entry("b200_commit_host_partials");
   B200_REQUIRE(out_partials != nullptr, "out_partials == nullptr");
   commit_on(g_state, curve_id, nullptr, num_sequences, descriptors, generators, offset_generators,
             out_partials);
@@ -1301,38 +1266,28 @@ void b200_fixed_msm_host_partials(void* out_partials, const struct sxt_multiexp_
                                   unsigned num_outputs, unsigned n, const uint8_t* scalars) {
   if (num_outputs == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_fixed_msm_host_partials");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h != nullptr && out_partials != nullptr, "null handle or out_partials");
+  const Entry entry("b200_fixed_msm_host_partials");
+  const HandleSet* h = handle_of(handle);
+  B200_REQUIRE(out_partials != nullptr, "out_partials == nullptr");
   fixed_host(nullptr, h, mode, element_num_bytes, output_bit_table, output_lengths, num_outputs, n,
              scalars, out_partials);
 }
 struct sxt_multiexp_handle* b200_multiexp_handle_new_device(unsigned curve_id,
                                                             const void* generators_dev,
                                                             unsigned n) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_multiexp_handle_new_device");
+  const Entry entry("b200_multiexp_handle_new_device");
   return reinterpret_cast<sxt_multiexp_handle*>(handle_new(curve_id, generators_dev, n, true));
 }
 void b200_combine_partials_device(unsigned curve_id, void* out_commitments, const void* partials,
                                   uint32_t num_parts, uint32_t count) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_combine_partials_device");
-  const CurveVTable& V = curve_vtable(curve_id);
-  DevBuf<unsigned char> sum((size_t)count * V.point_bytes, g_state.stream);
-  V.sum_parts(ctx(), partials, num_parts, count, sum.p);
-  V.store(ctx(), sum.p, out_commitments, count, true);
+  const Entry entry("b200_combine_partials_device");
+  combine_partials(curve_id, out_commitments, partials, num_parts, count, true);
 }
 void b200_combine_partials_projective_device(unsigned curve_id, void* out_res,
                                              const void* partials, uint32_t num_parts,
                                              uint32_t count) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_combine_partials_projective_device");
-  const CurveVTable& V = curve_vtable(curve_id);
-  DevBuf<unsigned char> sum((size_t)count * V.point_bytes, g_state.stream);
-  V.sum_parts(ctx(), partials, num_parts, count, sum.p);
-  V.store(ctx(), sum.p, out_res, count, false);
+  const Entry entry("b200_combine_partials_projective_device");
+  combine_partials(curve_id, out_res, partials, num_parts, count, false);
 }
 void b200_fixed_msm_device(void* out_res, void* out_partials,
                            const struct sxt_multiexp_handle* handle, int mode,
@@ -1341,35 +1296,24 @@ void b200_fixed_msm_device(void* out_res, void* out_partials,
                            const uint8_t* scalars) {
   if (num_outputs == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_fixed_msm_device");
-  const HandleSet* hs = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(hs != nullptr, "null handle");
+  const Entry entry("b200_fixed_msm_device");
+  const HandleSet* hs = handle_of(handle);
   B200_REQUIRE(hs->shards.size() == 1, "device-resident fixed MSM needs a single-device handle");
   const Handle* h = hs->shards[0];
-  unsigned rows = n;
-  if (mode == 2) {
-    rows = 0;
-    for (unsigned j = 0; j < num_outputs; ++j)
-      rows = output_lengths[j] > rows ? output_lengths[j] : rows;
-  }
   curve_vtable(h->curve_id).fixed_device(ctx(), out_res, out_partials, h, mode, element_num_bytes,
-                                         output_bit_table, output_lengths, num_outputs, rows,
-                                         scalars);
+                                         output_bit_table, output_lengths, num_outputs, n, scalars);
 }
 void b200_synthetic_generators_device(unsigned curve_id, void* out_generators, uint64_t n,
                                       uint64_t first, int projective) {
   if (n == 0)
     return;
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_synthetic_generators_device");
+  const Entry entry("b200_synthetic_generators_device");
   B200_REQUIRE(out_generators != nullptr, "out_generators == nullptr");
   curve_vtable(curve_id).synth_generators(ctx(), out_generators, n, first, projective != 0);
 }
 void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const void* generators_dev,
                                  uint64_t n, unsigned window_width) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_partition_table_device");
+  const Entry entry("b200_partition_table_device");
   const CurveVTable& V = curve_vtable(curve_id);
   const unsigned w = partition_window(window_width);
   if (n == 0)
@@ -1391,10 +1335,9 @@ void b200_partition_table_device(unsigned curve_id, void* out_table_dev, const v
 // writes chunk i - 1 to the file.
 void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle* handle,
                                                 const char* filename, unsigned window_width) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_multiexp_handle_write_partition_table");
-  const HandleSet* h = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(h && filename, "null handle or filename");
+  const Entry entry("b200_multiexp_handle_write_partition_table");
+  const HandleSet* h = handle_of(handle);
+  B200_REQUIRE(filename != nullptr, "null filename");
   const CurveVTable& V = curve_vtable(h->curve_id);
   const unsigned w = partition_window(window_width);
   cudaStream_t s = g_state.stream, sc = g_state.copy_stream;
@@ -1458,27 +1401,21 @@ void b200_multiexp_handle_write_partition_table(const struct sxt_multiexp_handle
 }
 unsigned b200_multiexp_handle_add_partition_table(struct sxt_multiexp_handle* handle,
                                                   unsigned window_width) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_multiexp_handle_add_partition_table");
-  HandleSet* hs = reinterpret_cast<HandleSet*>(handle);
-  B200_REQUIRE(hs != nullptr, "null handle");
-  return handle_add_partition_table(hs, window_width);
+  const Entry entry("b200_multiexp_handle_add_partition_table");
+  return handle_add_partition_table(handle_of(handle), window_width);
 }
 unsigned b200_multiexp_handle_partition_window(const struct sxt_multiexp_handle* handle) {
   std::lock_guard<std::mutex> lock(g_mutex);
-  const HandleSet* hs = reinterpret_cast<const HandleSet*>(handle);
-  B200_REQUIRE(hs != nullptr, "null handle");
+  const HandleSet* hs = handle_of(handle);
   return hs->shards.empty() ? 0u : hs->shards[0]->ptable_w;
 }
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_selftest_lane_arithmetic");
+  const Entry entry("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);
 }
 unsigned b200_selftest_sort(const sxt_sequence_descriptor* columns, unsigned num,
                             unsigned window_bits) {
-  std::lock_guard<std::mutex> lock(g_mutex);
-  require_init("b200_selftest_sort");
+  const Entry entry("b200_selftest_sort");
   B200_REQUIRE(num == 0 || columns != nullptr, "columns == nullptr");
   B200_REQUIRE(window_bits <= 20, "window_bits in 0..20");
   return selftest_sort(ctx(), columns, num, window_bits);

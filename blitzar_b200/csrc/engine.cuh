@@ -1,7 +1,7 @@
-// Device-level glue between the C ABI and the MSM engine: descriptor validation, column grouping,
-// generator ingestion, the choice between a handle's fixed-base table and the variable-base run
-// (prefer_table), result canonicalisation. Shared by api.cu (product) and the CPU-side emulation
-// harness under tests/emul (test infrastructure), both through the per-curve vtables.
+// Device-level glue between the C ABI and the MSM engine: column grouping, generator ingestion, the
+// choice between a handle's fixed-base table and the variable-base run (prefer_table), result
+// canonicalisation. Shared by api.cu (product) and the CPU-side emulation harness under tests/emul
+// (test infrastructure), both through the per-curve vtables.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -13,24 +13,6 @@
 #include "synth.cuh"
 
 namespace b200 {
-
-// validates like cbindings/pedersen.cc:44-68 and returns the longest column
-inline uint64_t check_descriptors(const sxt_sequence_descriptor* d, uint32_t num) {
-  B200_REQUIRE(d != nullptr, "descriptors == nullptr");
-  uint64_t longest = 0;
-  for (uint32_t i = 0; i < num; ++i) {
-    B200_REQUIRE(d[i].n == 0 || d[i].data != nullptr, "descriptor.n > 0 with data == nullptr");
-    B200_REQUIRE(d[i].element_nbytes != 0 && d[i].element_nbytes <= 32,
-                 "descriptor.element_nbytes must be in 1..32");
-    if (d[i].is_signed)
-      B200_REQUIRE(d[i].element_nbytes <= 16 &&
-                       (d[i].element_nbytes & (d[i].element_nbytes - 1)) == 0,
-                   "signed columns need a power-of-two element_nbytes <= 16");
-    B200_REQUIRE(d[i].n < (1ull << 31), "column too long");
-    longest = longest < d[i].n ? d[i].n : longest;
-  }
-  return longest;
-}
 
 // All kernel launches of one curve live behind CurveOps<C>, so each curve is instantiated in its
 // own translation unit (curve_*.cu) and api.cu only sees `extern template` declarations.
@@ -312,17 +294,7 @@ template <class C> struct CurveOps {
                            const uint8_t* scalars_dev) {
     stream_t s = ctx.s;
     std::vector<ColumnDesc> cols(num_outputs);
-    uint64_t row_bits = 0;
-    if (mode == 0) {
-      B200_REQUIRE(element_num_bytes >= 1 && element_num_bytes <= 32, "element_num_bytes in 1..32");
-      row_bits = 8ull * element_num_bytes * num_outputs;
-    } else {
-      for (unsigned j = 0; j < num_outputs; ++j) {
-        B200_REQUIRE(bit_table[j] > 0 && bit_table[j] <= 256, "output bit width must be in 1..256");
-        row_bits += bit_table[j];
-      }
-    }
-    const uint64_t row_stride = (row_bits + 7) / 8;
+    const uint64_t row_stride = fixed_row_bytes(mode, element_num_bytes, bit_table, num_outputs);
     uint64_t bit_off = 0;
     for (unsigned j = 0; j < num_outputs; ++j) {
       unsigned width = mode == 0 ? 8u * element_num_bytes : bit_table[j];

@@ -121,6 +121,41 @@ inline uint64_t range_begin(uint64_t n, uint32_t r, uint32_t num_ranges, int ske
 // for that range's copies)
 typedef void (*range_wait_fn)(void* user, uint64_t begin, uint64_t end);
 
+// validates like cbindings/pedersen.cc:44-68 and returns the longest column
+inline uint64_t check_descriptors(const sxt_sequence_descriptor* d, uint32_t num) {
+  B200_REQUIRE(d != nullptr, "descriptors == nullptr");
+  uint64_t longest = 0;
+  for (uint32_t i = 0; i < num; ++i) {
+    B200_REQUIRE(d[i].n == 0 || d[i].data != nullptr, "descriptor.n > 0 with data == nullptr");
+    B200_REQUIRE(d[i].element_nbytes != 0 && d[i].element_nbytes <= 32,
+                 "descriptor.element_nbytes must be in 1..32");
+    if (d[i].is_signed)
+      B200_REQUIRE(d[i].element_nbytes <= 16 &&
+                       (d[i].element_nbytes & (d[i].element_nbytes - 1)) == 0,
+                   "signed columns need a power-of-two element_nbytes <= 16");
+    B200_REQUIRE(d[i].n < (1ull << 31), "column too long");
+    longest = longest < d[i].n ? d[i].n : longest;
+  }
+  return longest;
+}
+
+// Bytes of one scalar row of a fixed-base call (mode 0 fixed width, 1 packed, 2 vlen): the outputs'
+// scalars side by side, element_num_bytes bytes each in mode 0, else bit_table[j] bits each.
+inline uint64_t fixed_row_bytes(int mode, unsigned element_num_bytes, const unsigned* bit_table,
+                                unsigned num_outputs) {
+  uint64_t row_bits = 0;
+  if (mode == 0) {
+    B200_REQUIRE(element_num_bytes >= 1 && element_num_bytes <= 32, "element_num_bytes in 1..32");
+    row_bits = 8ull * element_num_bytes * num_outputs;
+  } else {
+    for (unsigned j = 0; j < num_outputs; ++j) {
+      B200_REQUIRE(bit_table[j] > 0 && bit_table[j] <= 256, "output bit width must be in 1..256");
+      row_bits += bit_table[j];
+    }
+  }
+  return (row_bits + 7) / 8;
+}
+
 // Generator layout of a call whose column j pairs row i with generator offsets[j] + i (offsets null =
 // all 0). The intervals [offsets[j], offsets[j] + n_j) of the non-empty columns, merged where they
 // overlap or touch, are packed in increasing order into one array; column j's generator of row i

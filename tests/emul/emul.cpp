@@ -145,13 +145,8 @@ void emul_fixed(unsigned curve_id, void* res, const void* generators_proj, unsig
     h.ptable_w = partition_window;
     h.ptable_groups = groups;
   }
-  unsigned rows = n;
-  if (mode == 2) {
-    rows = 0;
-    for (unsigned j = 0; j < num_outputs; ++j) rows = std::max(rows, lengths[j]);
-  }
   V.fixed_device(ctx, res, nullptr, &h, mode, element_num_bytes, bit_table, lengths, num_outputs,
-                 rows, scalars);
+                 n, scalars);
 }
 
 // the outputs partition_route sends to a table of width window_width for outputs of the given
