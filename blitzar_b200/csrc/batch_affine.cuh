@@ -25,7 +25,17 @@
 
 namespace b200 {
 
-constexpr u32 kPadIndex = 0x7fffffffu;  // generator index of a pad entry (identity)
+// A sorted entry (DESIGN §3) is (key << 32) | (generator index << 1) | negate: sorting entries by
+// value sorts them by key. A pad entry (generator index kPadIndex) stands for the identity.
+constexpr u32 kPadIndex = 0x7fffffffu;
+B200_HD u64 make_entry(u32 key, u32 gen, bool negate) {
+  return ((u64)key << 32) | (u64)((gen << 1) | (negate ? 1u : 0u));
+}
+B200_HD u64 pad_entry(u32 key) { return make_entry(key, kPadIndex, false); }
+B200_HD u32 entry_key(u64 e) { return (u32)(e >> 32); }
+B200_HD u32 entry_gen(u64 e) { return (u32)e >> 1; }
+B200_HD bool entry_negate(u64 e) { return ((u32)e & 1u) != 0; }
+
 constexpr u32 kBatchGroup = 8;          // arity of the inversion tree: short serial chains per thread, the
                                         // levels above the first are latency-bound either way
 constexpr u32 kBatchTop = 4;            // at most this many values reach the top of the tree (their
@@ -116,14 +126,14 @@ template <class C> struct PairLevel {
       return;
     }
     const u64 ent = entries[slot];
-    const u32 idx = (u32)ent >> 1;
+    const u32 idx = entry_gen(ent);
     if (idx == kPadIndex) {
       a.x = F::zero();
       a.y = F::zero();
       return;
     }
     a = gens[idx];
-    if (((u32)ent & 1u) && !C::gen_is_identity(a))
+    if (entry_negate(ent) && !C::gen_is_identity(a))
       F::neg(a.y, a.y);
   }
   // 0 = chord addition, 1 = result is a, 2 = result is b, 3 = tangent (doubling), 4 = identity
@@ -163,8 +173,7 @@ template <class C> struct PairPass1Body {
     const u64 b = t * lv.B, e = b + lv.B < np ? b + lv.B : np;
     fe acc = F::one();
     for (u64 p = b; p < e; ++p) {
-      const u64 ea = lv.entries[2 * p], eb = lv.entries[2 * p + 1];
-      const u32 ia = (u32)ea >> 1, ib = (u32)eb >> 1;
+      const u32 ia = entry_gen(lv.entries[2 * p]), ib = entry_gen(lv.entries[2 * p + 1]);
       fe den = F::one();
       if (ia != kPadIndex && ib != kPadIndex) {
         const fe xa = lv.gens[ia].x, xb = lv.gens[ib].x;
@@ -301,7 +310,7 @@ struct FillPadsBody {
   const u32* cursor;  // end of the real entries of every bucket (scatter cursor)
   u64* entries;
   B200_HD void operator()(u64 k) const {
-    const u64 pad = ((u64)k << 32) | ((u64)kPadIndex << 1);
+    const u64 pad = pad_entry((u32)k);
     for (u32 i = cursor[k]; i < starts[k + 1]; ++i)
       entries[i] = pad;
   }
@@ -320,13 +329,13 @@ struct FinalEntriesBody {
     if (j == 0)
       *m_out = (u32)m;
     if (j < m)
-      entries[j] = (entries0[j << L] & 0xffffffff00000000ull) | (j << 1);
+      entries[j] = make_entry(entry_key(entries0[j << L]), (u32)j, false);
   }
 };
 
 template <class C> struct WalkInput {  // what the chunk walk (msm.cuh) sums
   const typename C::Gen* gens;
-  const u64* entries;  // (key << 32) | (index into gens << 1) | negate
+  const u64* entries;  // sorted entries, generator indices into gens
   const u32* m_ptr;    // number of entries (device)
   u64 m_max;           // bound on *m_ptr
 };

@@ -142,24 +142,8 @@ B200_HD void for_each_digit(const u32 v[8], bool negative, const ColumnDesc& col
   const u32 W = only_window == kAllWindows
                     ? col.num_windows
                     : (only_window < col.num_windows ? only_window + 1 : 0u);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    buf |= (u64)v[k] << nb;
-    nb += 32;
-    while (nb >= c && w < W) {
-      u32 d = ((u32)buf & mask) + carry;
-      buf >>= c;
-      nb -= c;
-      bool dneg = d > half;
-      carry = dneg ? 1u : 0u;
-      if (dneg)
-        d = (1u << c) - d;
-      if (d && (only_window == kAllWindows || w == only_window))
-        f((col.first_window + (col.table_n ? 0u : w)) * nbuckets + (d - 1u), negative != dneg, w);
-      ++w;
-    }
-  }
-  while (w < W) {
+  // digit of window w from the low c bits of buf
+  const auto step = [&] {
     u32 d = ((u32)buf & mask) + carry;
     buf >>= c;
     bool dneg = d > half;
@@ -169,7 +153,16 @@ B200_HD void for_each_digit(const u32 v[8], bool negative, const ColumnDesc& col
     if (d && (only_window == kAllWindows || w == only_window))
       f((col.first_window + (col.table_n ? 0u : w)) * nbuckets + (d - 1u), negative != dneg, w);
     ++w;
+  };
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    buf |= (u64)v[k] << nb;
+    nb += 32;
+    for (; nb >= c && w < W; nb -= c)
+      step();
   }
+  while (w < W)
+    step();
 }
 
 // ---- kernels (index-parallel bodies) -------------------------------------------------------------
@@ -186,6 +179,24 @@ B200_HD u32 column_of(const u64* col_start, u32 ncols, u64 tid) {
   }
   return lo;
 }
+// f(key, entry) for every non-zero digit of term tid (only_window as for_each_digit)
+template <class Fn>
+B200_HD void for_each_entry(const ColumnDesc* cols, const u64* col_start, u32 ncols, u32 c,
+                            u32 nbuckets, u64 tid, Fn f, u32 only_window = kAllWindows) {
+  const u32 j = column_of(col_start, ncols, tid);
+  const ColumnDesc col = cols[j];
+  if (only_window != kAllWindows && only_window >= col.num_windows)
+    return;
+  const u64 i = tid - col_start[j];
+  u32 v[8];
+  bool neg;
+  load_scalar_bits(v, neg, col, i);
+  const u32 ii = (u32)i + col.gen_base, tn = col.table_n;
+  for_each_digit(v, neg, col, c, nbuckets, [&](u32 key, bool negate, u32 w) {
+    f(key, make_entry(key, ii + w * tn, negate));
+  }, only_window);
+}
+
 struct CountBody {
   static constexpr int kBlock = 256;
   const ColumnDesc* cols;
@@ -193,14 +204,9 @@ struct CountBody {
   u32 ncols, c, nbuckets;
   u32* counts;
   B200_HD void operator()(u64 tid) const {
-    const u32 j = column_of(col_start, ncols, tid);
-    const ColumnDesc col = cols[j];
-    u64 i = tid - col_start[j];
-    u32 v[8];
-    bool neg;
-    load_scalar_bits(v, neg, col, i);
     u32* cnt = counts;
-    for_each_digit(v, neg, col, c, nbuckets, [cnt](u32 key, bool, u32) { B200_ATOMIC_ADD(&cnt[key], 1u); });
+    for_each_entry(cols, col_start, ncols, c, nbuckets, tid,
+                   [cnt](u32 key, u64) { B200_ATOMIC_ADD(&cnt[key], 1u); });
   }
 };
 
@@ -210,7 +216,7 @@ struct ScatterBody {
   const u64* col_start;
   u32 ncols, c, nbuckets;
   u32* cursor;  // exclusive offsets, consumed
-  u64* entries;  // (key << 32) | (generator index << 1) | negate
+  u64* entries;
   // window-major order (total_terms != 0): thread = (window, term), all threads of one window run
   // together, so the 8-byte scatter writes of a launch wave land in ONE window's slice of the entry
   // array (n x 8 B) and merge in L2 before they reach HBM, instead of spreading over all windows
@@ -221,21 +227,10 @@ struct ScatterBody {
       only = (u32)(tid / total_terms);
       tid -= (u64)only * total_terms;
     }
-    const u32 j = column_of(col_start, ncols, tid);
-    const ColumnDesc col = cols[j];
-    if (only != kAllWindows && only >= col.num_windows)
-      return;
-    u64 i = tid - col_start[j];
-    u32 v[8];
-    bool neg;
-    load_scalar_bits(v, neg, col, i);
     u32* cur = cursor;
     u64* en = entries;
-    const u32 ii = (u32)i + col.gen_base, tn = col.table_n;
-    for_each_digit(v, neg, col, c, nbuckets, [cur, en, ii, tn](u32 key, bool negate, u32 w) {
-      u32 pos = B200_ATOMIC_ADD(&cur[key], 1u);
-      en[pos] = ((u64)key << 32) | (u64)(((ii + w * tn) << 1) | (negate ? 1u : 0u));
-    }, only);
+    for_each_entry(cols, col_start, ncols, c, nbuckets, tid,
+                   [cur, en](u32 key, u64 e) { en[B200_ATOMIC_ADD(&cur[key], 1u)] = e; }, only);
   }
 };
 
@@ -349,22 +344,6 @@ template <int kBlock> __device__ u32 block_exclusive_scan(u32 v, u32* warp_sums,
   *total = warp_sums[kBlock / 32 - 1];
   __syncthreads();  // warp_sums may be reused right away
   return pre;
-}
-
-// f(key, entry) for every non-zero digit of term tid (entry as ScatterBody writes it)
-template <class Fn>
-__device__ void for_each_entry(const ColumnDesc* cols, const u64* col_start, u32 ncols, u32 c,
-                               u32 nbuckets, u64 tid, Fn f) {
-  const u32 j = column_of(col_start, ncols, tid);
-  const ColumnDesc col = cols[j];
-  const u64 i = tid - col_start[j];
-  u32 v[8];
-  bool neg;
-  load_scalar_bits(v, neg, col, i);
-  const u32 ii = (u32)i + col.gen_base, tn = col.table_n;
-  for_each_digit(v, neg, col, c, nbuckets, [&](u32 key, bool negate, u32 w) {
-    f(key, ((u64)key << 32) | (u64)(((ii + w * tn) << 1) | (negate ? 1u : 0u)));
-  });
 }
 
 struct MicroCountBody {
@@ -501,7 +480,7 @@ struct CoarseScatterBody {
     __syncthreads();
     for (u32 i = threadIdx.x; i < size; i += kBlock) {
       const u64 e = stage[i];
-      tmp[delta[__ldg(&map[(u32)(e >> 32) >> sh])] + i] = e;  // u32 wrap-around: slot < 2^32
+      tmp[delta[__ldg(&map[entry_key(e) >> sh])] + i] = e;  // u32 wrap-around: slot < 2^32
     }
   }
 };
@@ -537,7 +516,7 @@ struct BinSortBody {
     __syncthreads();
     for (u32 i = threadIdx.x; i < size; i += kBlock) {
       const u64 e = local ? ent[i] : tmp[(u64)lo + i];
-      atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u);
+      atomicAdd(&h[entry_key(e) - (u32)klo], 1u);
     }
     __syncthreads();
     const u32 per = (span + kBlock - 1) / kBlock, k0 = min(threadIdx.x * per, span),
@@ -557,7 +536,7 @@ struct BinSortBody {
     if (!local) {
       for (u32 i = threadIdx.x; i < size; i += kBlock) {
         const u64 e = tmp[(u64)lo + i];
-        entries[(u64)lo + atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u)] = e;
+        entries[(u64)lo + atomicAdd(&h[entry_key(e) - (u32)klo], 1u)] = e;
       }
       return;
     }
@@ -566,7 +545,7 @@ struct BinSortBody {
     u64* sorted = ent + kBinCap;
     for (u32 i = threadIdx.x; i < size; i += kBlock) {
       const u64 e = ent[i];
-      sorted[atomicAdd(&h[(u32)(e >> 32) - (u32)klo], 1u)] = e;
+      sorted[atomicAdd(&h[entry_key(e) - (u32)klo], 1u)] = e;
     }
     __syncthreads();
     for (u32 i = threadIdx.x; i < size; i += kBlock)
@@ -641,19 +620,26 @@ template <class C> inline void fill_identity(stream_t s, typename C::Point* p, u
   launch(FillIdentityBody<C>{(uint4*)p}, n * FillIdentityBody<C>::kChunks, s);
 }
 
-// buckets[k] += scratch[k] for every bucket the current generator range touched (bucket_end = the
-// range's cursor array after the scatter). A later range accumulates into its own scratch array and
-// is merged here: one coalesced pass, instead of a read-add-write at every run boundary of the
-// accumulation kernel (about twice as fast per piece at C2 in 4 pieces).
+// The real entries of bucket k of a sorted range are the slots [begin(k), end(k)). A padded layout
+// keeps every bucket's start; in a dense one a bucket starts where the previous one ends.
+struct BucketOffsets {
+  const u32* ends;    // end offset of every bucket's real entries
+  const u32* starts;  // padded layouts: start offset of every bucket, nkeys + 1; null = dense layout
+  B200_HD u32 begin(u64 k) const { return starts ? starts[k] : (k ? ends[k - 1] : 0u); }
+  B200_HD u32 end(u64 k) const { return ends[k]; }
+};
+
+// buckets[k] += scratch[k] for every bucket the current generator range touched. A later range
+// accumulates into its own scratch array and is merged here: one coalesced pass, instead of a
+// read-add-write at every run boundary of the accumulation kernel (about twice as fast per piece at
+// C2 in 4 pieces).
 template <class C> struct MergeBucketsBody {
   static constexpr int kBlock = 128;
-  const u32* bucket_end;
-  const u32* bucket_begin;  // padded layouts: start offset of every bucket; null = dense layout
+  BucketOffsets offsets;
   const typename C::Point* scratch;
   typename C::Point* buckets;
   B200_HD void operator()(u64 k) const {
-    const u32 lo = bucket_begin ? bucket_begin[k] : (k ? bucket_end[k - 1] : 0u);
-    if (bucket_end[k] == lo)
+    if (offsets.begin(k) == offsets.end(k))
       return;
     typename C::Point b = buckets[k];
     C::add(b, b, scratch[k]);
@@ -682,7 +668,7 @@ struct AccumulateBody {
   typedef typename C::Point Point;
   typedef typename C::Gen Gen;
   const u32* keys;                 // level >= 2
-  const u64* entries;              // level 1: (key << 32) | (generator index << 1) | negate
+  const u64* entries;              // level 1: sorted entries
   const Gen* gens;                 // level 1
   const Point* pieces;             // level >= 2
   const u32* m_ptr;                // number of entries at this level (device)
@@ -694,26 +680,19 @@ struct AccumulateBody {
   u32* out_m_ptr;
   const u32* unit_veto;  // kUnitZ: device flag, non-zero = run the 8-multiplication path; may be null
 
-  // every bucket is written exactly once per generator range (a run strictly inside a chunk is
-  // complete; split runs travel down the cascade and are written by the level that completes them)
-  B200_HD void put_bucket(u32 key, const Point& acc, bool writer) const {
-    if (writer)
-      buckets[key] = acc;
-  }
-  B200_HD u32 key_at(u64 i) const { return kGather ? (u32)(entries[i] >> 32) : keys[i]; }
-  B200_HD void fetch(Point& acc, u64 i, bool first) const {
-    if (kGather) {
-      u32 e = (u32)entries[i];
-      if (first)
-        C::gen_to_point(acc, gens[e >> 1], e & 1u);
-      else
-        C::template add_gen<X>(acc, acc, gens[e >> 1], e & 1u);
-    } else {
-      if (first)
-        acc = pieces[i];
-      else
-        C::template add<X>(acc, acc, pieces[i]);
+  // The run of `key` in chunk t ends with the sum acc. Every bucket is written exactly once per
+  // generator range: a run after the chunk's first is complete (it started inside the chunk), and so
+  // is every run of the final level; the first run may continue in the previous chunk, so it travels
+  // down the cascade as the chunk's first piece and is written by the level that completes it.
+  B200_HD void close_run(u64 t, u32 key, const Point& acc, bool writer, bool& first_seg) const {
+    if (final_level || !first_seg) {
+      if (writer)
+        buckets[key] = acc;
+    } else if (writer) {
+      out_keys[2 * t] = key;
+      out_pieces[2 * t] = acc;
     }
+    first_seg = false;
   }
   template <bool kUnit> B200_HD Gen load_gen(u32 idx) const {
     if constexpr (kUnit)
@@ -729,61 +708,40 @@ struct AccumulateBody {
     // addition of entry i starts, so the random 128-byte read overlaps ~1300 instructions of
     // field arithmetic instead of stalling the warp on the long scoreboard
     u64 ent = entries[b];
-    Gen g = load_gen<kUnit>((u32)ent >> 1);
-    cur = (u32)(ent >> 32);
-    struct {
-      Point p;
-      B200_HD void start(const Gen& g, bool negate) { C::gen_to_point(p, g, negate); }
-      B200_HD void add(const Gen& g, bool negate) {
-        C::template add_gen<X>(p, p, g, negate, kUnit);
-      }
-      B200_HD void get(Point& out) const { out = p; }
-    } ga;
+    Gen g = load_gen<kUnit>(entry_gen(ent));
+    cur = entry_key(ent);
     for (u64 i = b; i < e; ++i) {
       u64 ent_n = ent;
       Gen g_n = g;
       if (i + 1 < e) {
         ent_n = entries[i + 1];
-        g_n = load_gen<kUnit>((u32)ent_n >> 1);
+        g_n = load_gen<kUnit>(entry_gen(ent_n));
       }
-      const u32 k = (u32)(ent >> 32);
-      const bool negate = ((u32)ent & 1u) != 0;
+      const u32 k = entry_key(ent);
+      const bool negate = entry_negate(ent);
       if (kUniform) {
-        if (i == b) {
-          ga.p = C::identity();
-        } else if (k != cur) {
-          ga.get(acc);
-          if (final_level || !first_seg) {
-            put_bucket(cur, acc, writer);
-          } else if (writer) {
-            out_keys[2 * t] = cur;
-            out_pieces[2 * t] = acc;
+        if (i == b || k != cur) {
+          if (i != b) {
+            close_run(t, cur, acc, writer, first_seg);
+            cur = k;
           }
-          first_seg = false;
-          cur = k;
-          ga.p = C::identity();
+          acc = C::identity();
         }
-        ga.add(g, negate);
-      } else if (i == b) {
-        ga.start(g, negate);
-      } else if (k == cur) {
-        ga.add(g, negate);
+        C::template add_gen<X>(acc, acc, g, negate, kUnit);
       } else {
-        ga.get(acc);
-        if (final_level || !first_seg) {
-          put_bucket(cur, acc, writer);
-        } else if (writer) {
-          out_keys[2 * t] = cur;
-          out_pieces[2 * t] = acc;
+        const bool start = i == b || k != cur;
+        if (k != cur) {
+          close_run(t, cur, acc, writer, first_seg);
+          cur = k;
         }
-        first_seg = false;
-        cur = k;
-        ga.start(g, negate);
+        if (start)
+          C::gen_to_point(acc, g, negate);
+        else
+          C::template add_gen<X>(acc, acc, g, negate, kUnit);
       }
       ent = ent_n;
       g = g_n;
     }
-    ga.get(acc);
   }
   B200_HD void operator()(u64 tid) const {
     const u64 t = tid / X::kLanes;
@@ -799,76 +757,50 @@ struct AccumulateBody {
     u32 cur;
     Point acc;
     bool first_seg = true;
-    if (kGather) {
+    if constexpr (kGather) {
       if (kUnitZ && unit_veto && *unit_veto)
         gather_walk<false>(t, b, e, writer, cur, acc, first_seg);
       else
         gather_walk<kUnitZ>(t, b, e, writer, cur, acc, first_seg);
     } else {
-      cur = key_at(b);
-      fetch(acc, b, true);
+      cur = keys[b];
+      acc = pieces[b];
       for (u64 i = b + 1; i < e; ++i) {
-        u32 k = key_at(i);
+        const u32 k = keys[i];
         if (k == cur) {
-          fetch(acc, i, false);
+          C::template add<X>(acc, acc, pieces[i]);
         } else {
-          if (final_level || !first_seg) {
-            put_bucket(cur, acc, writer);
-          } else if (writer) {
-            out_keys[2 * t] = cur;
-            out_pieces[2 * t] = acc;
-          }
-          first_seg = false;
+          close_run(t, cur, acc, writer, first_seg);
           cur = k;
-          fetch(acc, i, true);
+          acc = pieces[i];
         }
       }
     }
     if (final_level) {
-      put_bucket(cur, acc, writer);
+      close_run(t, cur, acc, writer, first_seg);
       return;
     }
     if (!writer)
       return;
-    if (first_seg) {  // single-segment chunk: pad the tail slot with the identity
-      out_keys[2 * t] = cur;
-      out_pieces[2 * t] = acc;
-      out_keys[2 * t + 1] = cur;
-      out_pieces[2 * t + 1] = C::identity();
-    } else {
-      out_keys[2 * t + 1] = cur;
-      out_pieces[2 * t + 1] = acc;
+    if (first_seg) {  // single-run chunk: it is the first piece, the identity pads the second
+      close_run(t, cur, acc, writer, first_seg);
+      acc = C::identity();
     }
+    out_keys[2 * t + 1] = cur;
+    out_pieces[2 * t + 1] = acc;
   }
 };
 
-// window_used[w] |= (some entry of this pass landed in window w); bucket_end = cursor array after
-// the scatter (end offset of every bucket)
+// window_used[w] |= (some entry of this pass landed in window w). A bucket is padded to zero slots
+// exactly when it has no entry, so the padded offsets answer this as well as the dense ones.
 struct WindowUsedBody {
   static constexpr int kBlock = 64;
-  const u32* bucket_end;
+  BucketOffsets offsets;
   u32 nbuckets;
   u32* window_used;
   B200_HD void operator()(u64 w) const {
-    u32 lo = w ? bucket_end[w * nbuckets - 1] : 0u;
-    u32 hi = bucket_end[(w + 1) * nbuckets - 1];
-    if (hi != lo)
+    if (offsets.begin(w * nbuckets) != offsets.begin((w + 1) * nbuckets))
       window_used[w] = 1u;
-  }
-};
-
-// same flag from the per-bucket counts (before they are padded / scanned): thread t looks at 256 buckets
-struct WindowUsedFromCountsBody {
-  static constexpr int kBlock = 128;
-  const u32* counts;
-  u64 nkeys;
-  u32 nbuckets;
-  u32* window_used;
-  B200_HD void operator()(u64 t) const {
-    const u64 b = t * 256, e = b + 256 < nkeys ? b + 256 : nkeys;
-    for (u64 k = b; k < e; ++k)
-      if (counts[k])
-        window_used[k / nbuckets] = 1u;
   }
 };
 
@@ -1520,13 +1452,14 @@ struct StagedRange {
 };
 
 struct SortedLayout {  // the sorted (term, window) entries of one range, read by every later stage
-  u64* entries;   // sorted by key, (key << 32) | (generator index << 1) | negate; with L > 0 every
-                  // bucket is followed by pad entries (index kPadIndex) up to a multiple of 2^L slots
+  u64* entries;   // sorted entries; with L > 0 every bucket is followed by pad entries up to a
+                  // multiple of 2^L slots
   u32* counts;    // [nkeys + 1]: counts[k] = END offset of bucket k's real entries
   u32* starts;    // [nkeys + 1]: padded start offset of every bucket; null when L = 0
   u32* d_m;       // [16]: d_m[0] = number of slots; the rest is scratch of the later stages
   u64 slots_max;  // slots allocated for `entries` (bound on d_m[0])
   bool binned;    // sorted by the binned path
+  BucketOffsets offsets() const { return {counts, starts}; }
 };
 
 // Sorts a staged range into a SortedLayout and flags window_used[w] for every window with an entry.
@@ -1552,10 +1485,8 @@ inline SortedLayout sort_entries(stream_t s, const MsmPlan& plan, const StagedRa
   if (!out.binned) {
     dev_zero(out.counts, (nkeys + 1) * sizeof(u32), s);
     launch(CountBody{r.d_cols, r.d_col_start, ncols, c, nbuckets, out.counts}, total_terms, s);
-    if (L) {
-      launch(WindowUsedFromCountsBody{out.counts, nkeys, nbuckets, window_used}, (nkeys + 255) / 256, s);
+    if (L)
       launch(PadCountsBody{out.counts, (1u << L) - 1u}, nkeys, s);
-    }
     exclusive_scan(out.counts, nkeys + 1, s);  // counts[nkeys] = number of (padded) entries
     copy_d2d(out.d_m, out.counts + nkeys, sizeof(u32), s);
     if (L) {
@@ -1569,8 +1500,7 @@ inline SortedLayout sort_entries(stream_t s, const MsmPlan& plan, const StagedRa
   }
   if (L)
     launch(FillPadsBody{out.starts, out.counts, out.entries}, nkeys, s);
-  else
-    launch(WindowUsedBody{out.counts, nbuckets, window_used}, plan.total_windows, s);
+  launch(WindowUsedBody{out.offsets(), nbuckets, window_used}, plan.total_windows, s);
   return out;
 }
 
@@ -1650,6 +1580,13 @@ stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, bool
     Point* out_pieces = final_level ? nullptr : (Point*)dev_alloc(2 * T * sizeof(Point), cs);
     to_free.insert(to_free.end(), {out_keys, out_pieces});
     u32* out_m = d_m + 1 + (level % 8);
+    // `body` only names the AccumulateBody instantiation: every level gets the same fields and reads
+    // the ones it needs
+    const auto launch_level = [&](auto body, u64 threads, stream_t st) {
+      body = {lvl_keys, walk.entries, walk.gens, lvl_pieces, walk.m_ptr, K, final_level, target,
+              out_keys, out_pieces, out_m, unit_veto};
+      launch(body, threads, st);
+    };
     if (level == 0) {
       // faster on ed25519 (a run start is a multiplication by a constant there); the Weierstrass
       // start is free, so the extra addition loses
@@ -1659,37 +1596,21 @@ stream_t chunk_walk(stream_t s, stream_t tail, WalkInput<C> walk, u32* d_m, bool
       constexpr bool kEd = C::kCurveId == kRistretto255;
       const bool unit_path = kEd && unit;
       if (uniform && unit_path)
-        launch(AccumulateBody<C, true, SeqExec, true, kEd>{nullptr, walk.entries, walk.gens, nullptr,
-                                                            walk.m_ptr, K, final_level, target,
-                                                            out_keys, out_pieces, out_m, unit_veto},
-               T, s);
+        launch_level(AccumulateBody<C, true, SeqExec, true, kEd>{}, T, s);
       else if (uniform)
-        launch(AccumulateBody<C, true, SeqExec, true>{nullptr, walk.entries, walk.gens, nullptr,
-                                                      walk.m_ptr, K, final_level, target, out_keys,
-                                                      out_pieces, out_m, nullptr},
-               T, s);
+        launch_level(AccumulateBody<C, true, SeqExec, true>{}, T, s);
       else if (unit_path)
-        launch(AccumulateBody<C, true, SeqExec, false, kEd>{nullptr, walk.entries, walk.gens, nullptr,
-                                                             walk.m_ptr, K, final_level, target,
-                                                             out_keys, out_pieces, out_m, unit_veto},
-               T, s);
+        launch_level(AccumulateBody<C, true, SeqExec, false, kEd>{}, T, s);
       else
-        launch(AccumulateBody<C, true>{nullptr, walk.entries, walk.gens, nullptr, walk.m_ptr, K,
-                                       final_level, target, out_keys, out_pieces, out_m, nullptr},
-               T, s);
+        launch_level(AccumulateBody<C, true>{}, T, s);
       KernelTimer::get().end(s);
       if (tail != s)
         stream_follow(tail, s);
       cs = tail;
     } else if (T <= opt.quad_threshold) {
-      launch(AccumulateBody<C, false, QuadExec>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr,
-                                                K, final_level, target, out_keys, out_pieces, out_m,
-                                                nullptr},
-             T * QuadExec::kLanes, cs);
+      launch_level(AccumulateBody<C, false, QuadExec>{}, T * QuadExec::kLanes, cs);
     } else {
-      launch(AccumulateBody<C, false>{lvl_keys, nullptr, nullptr, lvl_pieces, walk.m_ptr, K,
-                                      final_level, target, out_keys, out_pieces, out_m, nullptr},
-             T, cs);
+      launch_level(AccumulateBody<C, false>{}, T, cs);
     }
     if (final_level)
       break;
@@ -1758,7 +1679,7 @@ void msm_accumulate_range(stream_t s, const MsmPlan& plan, const typename C::Gen
   // freed on s, it could go to the next range's allocations while cs still reads it. So are the last
   // pair level's points and entries. The sorted entries and the staged columns are read on s only.
   if (add_into) {
-    launch(MergeBucketsBody<C>{sorted.counts, sorted.starts, target, d_buckets}, nkeys, cs);
+    launch(MergeBucketsBody<C>{sorted.offsets(), target, d_buckets}, nkeys, cs);
     dev_free(target, cs);
   }
   to_free.insert(to_free.end(), {sorted.d_m, sorted.counts, sorted.starts});
