@@ -386,11 +386,21 @@ def commit_host_partials(curve_id, columns, generators, out_partial_ptr, offset_
 
 
 def fixed_msm_device(handle, out_res_ptr, out_partial_ptr, element_num_bytes, num_outputs, n,
-                     scalars_ptr):
-    """b200_fixed_msm_device, fixed-width mode."""
+                     scalars_ptr, bit_table=None, lengths=None):
+    """b200_fixed_msm_device: fixed-width mode, packed mode with bit_table, or vlen mode with
+    bit_table and lengths (one entry per output each)."""
+    mode, bt, ol = 0, None, None
+    if bit_table is not None:
+        if len(bit_table) != num_outputs or (lengths is not None and len(lengths) != num_outputs):
+            raise ValueError(f"bit_table and lengths must hold one entry per output ({num_outputs})")
+        mode = 1 if lengths is None else 2
+        bt = (C.c_uint * num_outputs)(*bit_table)
+        ol = None if lengths is None else (C.c_uint * num_outputs)(*lengths)
+    elif lengths is not None:
+        raise ValueError("lengths need a bit_table")
     lib().b200_fixed_msm_device(C.c_void_p(out_res_ptr), C.c_void_p(out_partial_ptr),
-                                C.c_void_p(handle.h), C.c_int(0), C.c_uint(element_num_bytes),
-                                None, None, C.c_uint(num_outputs), C.c_uint(n),
+                                C.c_void_p(handle.h), C.c_int(mode), C.c_uint(element_num_bytes),
+                                bt, ol, C.c_uint(num_outputs), C.c_uint(n),
                                 C.c_void_p(scalars_ptr))
 
 

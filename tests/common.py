@@ -1,5 +1,15 @@
-"""Shared input builders for the parity tests (seeded, deterministic)."""
+"""Shared input builders for the parity tests (seeded, deterministic), and the runner of the cases
+that need a fresh interpreter."""
+import importlib
+import json
+import os
+import subprocess
+import sys
+
 import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 # the reference's end-to-end golden (rust/tests/src/main.rs:21-49): three u32 columns over the
 # built-in generators at offset 0 and their ristretto255 commitments
@@ -311,3 +321,47 @@ def mt19937_bytes(seed, n, nbytes=32, top_mask=0x0F):
     out = (rs.randint(0, 2 ** 32, n * nbytes, dtype=np.uint64) >> 24).astype(np.uint8).reshape(n, nbytes)
     out[:, nbytes - 1] &= top_mask
     return out
+
+
+# ---- cases that need a fresh interpreter -------------------------------------------------------------
+# The library reads part of its configuration once per process: sxt_init's arguments,
+# BLITZAR_B200_DEVICES / _SHARED_DEVICES, BLITZAR_B200_MIN_SHARD_TERMS and BLITZAR_LOG_LEVEL. A child
+# gets none of the variables the library reads from the test process, only the ones the case sets.
+_LIBRARY_ENV = ("BLITZAR_LOG_LEVEL", "BLITZAR_PARTITION_WINDOW_WIDTH", "BLITZAR_BACKEND")
+_FRESH_DONE = "fresh process: every body returned"
+_FRESH_CHILD = ("import sys; sys.path.insert(0, sys.argv[1]); from tests import common; "
+                "common._fresh_child(sys.argv[2])")
+
+
+def run_fresh(*bodies, init={"num_precomputed_generators": 64}, env=None):
+    """Runs body(bb, port, *args) for each entry, in order, in one new interpreter and returns its
+    CompletedProcess. An entry is a module-level function or a tuple (function, *args) with
+    JSON-serialisable args; the child imports the function by module and name. init: the child's
+    sxt_init arguments (None: the child leaves the library alone). env: variables set on top of this
+    process's environment without the library's variables."""
+    calls = []
+    for entry in bodies:
+        fn, *args = entry if isinstance(entry, tuple) else (entry,)
+        calls.append((fn.__module__, fn.__qualname__, args))
+    child_env = {k: v for k, v in os.environ.items()
+                 if not (k.startswith("BLITZAR_B200_") or k in _LIBRARY_ENV)}
+    child_env.update(env or {})
+    r = subprocess.run([sys.executable, "-c", _FRESH_CHILD, ROOT,
+                        json.dumps(dict(init=init, calls=calls))],
+                       env=child_env, cwd=ROOT, capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0 and _FRESH_DONE in r.stdout, r.stdout + r.stderr[-8000:]
+    return r
+
+
+def _fresh_child(spec):
+    import blitzar_b200 as bb
+    from oracle import port
+    spec = json.loads(spec)
+    calls = [(getattr(importlib.import_module(module), name), args)
+             for module, name, args in spec["calls"]]
+    port.build()
+    if spec["init"] is not None:
+        assert bb.sxt_init(**spec["init"]) == 0
+    for fn, args in calls:
+        fn(bb, port, *args)
+    print(_FRESH_DONE)

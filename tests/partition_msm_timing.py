@@ -13,7 +13,6 @@ has taken 25 minutes; both are printed as "not measured". The results of the thr
 compared on the host for every shape. Prints the card's name, power limit and SM clock first, then
 one markdown row per shape; also writes the rows as JSON to out_dir.
     python tests/partition_msm_timing.py [out_dir]"""
-import ctypes as C
 import json
 import os
 import statistics
@@ -25,7 +24,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 
 import blitzar_b200 as bb  # noqa: E402
-from blitzar_b200.api import lib  # noqa: E402
 from oracle import port  # noqa: E402
 
 CURVES = {0: "ristretto255", 2: "bn254"}
@@ -44,22 +42,15 @@ def card():
         return "unknown card"
 
 
-def device_call(h, mode, bt, lens, m, n, out, sc):
-    lib().b200_fixed_msm_device(C.c_void_p(out.ptr), None, C.c_void_p(h.h), C.c_int(mode),
-                                C.c_uint(0), (C.c_uint * m)(*bt),
-                                (C.c_uint * m)(*lens) if lens else None, C.c_uint(m), C.c_uint(n),
-                                C.c_void_p(sc.ptr))
-
-
-def measure(h, mode, bt, lens, m, n, out, sc, psc, policy):
+def measure(h, bt, lens, m, n, out, sc, psc, policy):
     os.environ["BLITZAR_B200_PARTITION_POLICY"] = str(policy)
-    device_call(h, mode, bt, lens, m, n, out, sc)
+    bb.fixed_msm_device(h, out.ptr, None, 0, m, n, sc.ptr, bit_table=bt, lengths=lens)
     bb.synchronize()
     times = []
     for _ in range(3):
         e0, e1 = bb.Event(), bb.Event()
         e0.record()
-        device_call(h, mode, bt, lens, m, n, out, sc)
+        bb.fixed_msm_device(h, out.ptr, None, 0, m, n, sc.ptr, bit_table=bt, lengths=lens)
         e1.record()
         times.append(e0.elapsed_ms(e1))
     res = out.to_host()
@@ -110,7 +101,7 @@ def main():
                         sc = bb.DeviceBuffer(host=np.concatenate([psc.reshape(-1),
                                                                   np.zeros(64, np.uint8)]))
                         out = bb.DeviceBuffer(m * PROJ[curve])
-                        r = {p: measure(h, 2 if lens else 1, bt, lens, m, n, out, sc, psc, p)
+                        r = {p: measure(h, bt, lens, m, n, out, sc, psc, p)
                              for p in (2, 1, 0)}
                         ref = port.normalize(curve, r[2][4].reshape(m, PROJ[curve]))
                         same = all(np.array_equal(port.normalize(curve, r[p][4].reshape(m, PROJ[curve])),

@@ -7,7 +7,8 @@ import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.common import ROOT
+
 HEADER = os.path.join(ROOT, "include", "blitzar_b200.h")
 
 

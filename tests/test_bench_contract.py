@@ -5,7 +5,7 @@ import os
 import subprocess
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.common import ROOT
 
 
 def test_reference_arm_prints_one_contract_line(refcpu):

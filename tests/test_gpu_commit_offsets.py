@@ -2,8 +2,6 @@
 with_offsets, b200_commit_device_with_offsets): every column must equal the oracle's commitment of
 that column alone at its offset, and, at full size, k separate calls of the existing entry points."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -12,7 +10,6 @@ from tests import common
 from tests.test_commit_offsets import FAR, columns, lengths, offset_patterns, oracle
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _gens(port, curve, offsets, lens):
@@ -83,7 +80,6 @@ def test_forced_pair_levels(bb, port, curve, monkeypatch):
 def test_device_entry_partials_combined(bb, port, curve):
     """Rows [0, h) at offsets and rows [h, n) at offsets + h, as partial points combined on the device,
     equal the one-pass commitments (the MSM is linear)."""
-    import ctypes as C
     n, h = 900, 400
     cols = columns(240 + curve, n=n, shapes=[(0, 32, 0), (0, 8, 1), (-300, 16, 0)])
     lens = [n, n, n - 300]
@@ -104,8 +100,7 @@ def test_device_entry_partials_combined(bb, port, curve):
                                   [o + l for o, l in zip(offsets, lo)], None, parts.ptr + 3 * pb)
     stride = bb.CURVE_SIZES[curve][2]
     out = bb.DeviceBuffer(3 * stride)
-    bb.lib().b200_combine_partials_device(C.c_uint(curve), C.c_void_p(out.ptr), C.c_void_p(parts.ptr),
-                                          C.c_uint32(2), C.c_uint32(3))
+    bb.combine_partials_device(curve, out.ptr, parts.ptr, 2, 3)
     got = out.to_host((3, stride))
     assert common.same(curve, got, want)
     # out_commitments of one device call
@@ -117,67 +112,34 @@ def test_device_entry_partials_combined(bb, port, curve):
         b_.free()
 
 
-_MULTI_DEVICE = r"""
-import sys, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200.api as bb
-from oracle import port
-from tests import common
-from tests.test_commit_offsets import oracle
-port.build()
-assert bb.sxt_init(num_precomputed_generators=64) == 0
-rng = np.random.default_rng(5)
-for curve in range(4):
-    # by column (at least as many columns as devices), then by generator range (one column)
-    for n, shapes, offsets in ((700, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-699, 8, 0), (0, 4, 1)],
-                                [0, 900, 350, 5, 2000]),
-                               (1500, [(0, 32, 0)], [333])):
-        cols = common.random_columns(rng, n, shapes)
-        gens = common.generators_for(port, curve, max(offsets) + n)[0]
-        got = bb.compute_pedersen_commitments_with_offsets(curve, cols, offsets, gens)
-        assert common.same(curve, got, oracle(port, curve, cols, offsets, gens)), (curve, len(cols))
-        if curve == 0:
-            offs = [o + (1 << 33) for o in offsets]
-            got = bb.compute_pedersen_commitments_with_offsets(0, cols, offs)
-            assert np.array_equal(got, oracle(port, 0, cols, offs, None)), len(cols)
-print("multi-device offsets ok")
-"""
+# ---- fresh-process bodies, run by tests/test_gpu_parity.py next to the plain entry point's ---------
+def _fresh_split_over_devices(bb, port):
+    """BLITZAR_B200_DEVICES=k: by column and by generator range."""
+    rng = np.random.default_rng(5)
+    for curve in range(4):
+        # by column (at least as many columns as devices), then by generator range (one column)
+        for n, shapes, offsets in ((700, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-699, 8, 0), (0, 4, 1)],
+                                    [0, 900, 350, 5, 2000]),
+                                   (1500, [(0, 32, 0)], [333])):
+            cols = common.random_columns(rng, n, shapes)
+            gens = common.generators_for(port, curve, max(offsets) + n)[0]
+            got = bb.compute_pedersen_commitments_with_offsets(curve, cols, offsets, gens)
+            assert common.same(curve, got, oracle(port, curve, cols, offsets, gens)), (curve, len(cols))
+            if curve == 0:
+                offs = [o + (1 << 33) for o in offsets]
+                got = bb.compute_pedersen_commitments_with_offsets(0, cols, offs)
+                assert np.array_equal(got, oracle(port, 0, cols, offs, None)), len(cols)
 
 
-def test_split_over_devices():
-    import torch
-    env = dict(os.environ, BLITZAR_B200_DEVICES=str(max(2, min(4, torch.cuda.device_count()))),
-               BLITZAR_B200_SHARED_DEVICES="1" if torch.cuda.device_count() < 2 else "0",
-               BLITZAR_B200_MIN_SHARD_TERMS="200")
-    r = subprocess.run([sys.executable, "-c", _MULTI_DEVICE, ROOT], env=env, cwd=ROOT,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "multi-device offsets ok" in r.stdout, r.stdout + r.stderr
-
-
-_BUILTIN_TABLE = r"""
-import sys, os, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200.api as bb
-from oracle import port
-from tests import common
-from tests.test_commit_offsets import oracle
-port.build()
-assert bb.sxt_init(num_precomputed_generators=5000) == 0
-rng = np.random.default_rng(6)
-cols = common.random_columns(rng, 2000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-1999, 8, 0)])
-for policy in ("1", "2", "0"):
-    os.environ["BLITZAR_B200_TABLE_POLICY"] = policy
-    for offsets in ([0, 37, 1000, 2999], [0, 3500, 10, 4000], [5000, 6000, 9000, 5001]):
-        got = bb.compute_pedersen_commitments_with_offsets(0, cols, offsets)
-        assert np.array_equal(got, oracle(port, 0, cols, offsets, None)), (policy, offsets)
-print("builtin table offsets ok")
-"""
-
-
-def test_builtin_generator_table_subprocess():
-    r = subprocess.run([sys.executable, "-c", _BUILTIN_TABLE, ROOT], cwd=ROOT, capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0 and "builtin table offsets ok" in r.stdout, r.stdout + r.stderr
+def _fresh_builtin_generator_table(bb, port):
+    """num_precomputed_generators=5000: offsets inside, straddling and beyond the built-in table."""
+    rng = np.random.default_rng(6)
+    cols = common.random_columns(rng, 2000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-1999, 8, 0)])
+    for policy in ("1", "2", "0"):
+        os.environ["BLITZAR_B200_TABLE_POLICY"] = policy
+        for offsets in ([0, 37, 1000, 2999], [0, 3500, 10, 4000], [5000, 6000, 9000, 5001]):
+            got = bb.compute_pedersen_commitments_with_offsets(0, cols, offsets)
+            assert np.array_equal(got, oracle(port, 0, cols, offsets, None)), (policy, offsets)
 
 
 @pytest.mark.parametrize("curve", [0, 2])

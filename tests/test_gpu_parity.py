@@ -4,14 +4,14 @@ this path is integer / byte data. Modelled on cbindings/pedersen.t.cc:243-612,
 cbindings/fixed_pedersen.t.cc:45-200, get_generators.t.cc, get_one_commit.t.cc and the shared
 conformance suite sxt/multiexp/test/multiexponentiation.cc:42-451."""
 import os
+import tempfile
 
 import numpy as np
 import pytest
 
-from tests import common
+from tests import common, test_gpu_commit_offsets
 
 pytestmark = pytest.mark.gpu
-GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def test_native_library_is_loaded(bb):
@@ -28,11 +28,11 @@ def test_reference_golden_commitments(bb):
 
 def test_committed_reference_fixtures(bb, port):
     for curve in range(4):
-        z = np.load(os.path.join(GOLDEN_DIR, f"commit_curve{curve}.npz"))
+        z = np.load(os.path.join(common.GOLDEN, f"commit_curve{curve}.npz"))
         cols = [(z[f"col{j}"], int(z["signed"][j])) for j in range(len(z["signed"]))]
         out = bb.compute_pedersen_commitments(curve, cols, z["generators"])
         assert common.same(curve, out, z["commitments"]), curve
-        f = np.load(os.path.join(GOLDEN_DIR, f"fixed_curve{curve}.npz"))
+        f = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))
         h = bb.MultiexpHandle(curve, f["generators_p"])
         res = h.fixed_multiexponentiation(int(f["element_num_bytes"]), int(f["num_outputs"]),
                                           int(f["n"]), f["scalars"])
@@ -87,7 +87,6 @@ def test_random_sweep(bb, port, curve, n):
 
 def test_skewed_digits_and_tuning(bb, port):
     """All terms in one bucket; every window width; odd chunk shapes (cascade depth)."""
-    import ctypes as C
     rng = np.random.default_rng(8)
     n = 6000
     gens, _ = common.generators_for(port, 0, n)
@@ -97,10 +96,10 @@ def test_skewed_digits_and_tuning(bb, port):
     want = port.commit(0, cols, gens)
     try:
         for c, k1, kn in [(2, 32, 8), (5, 7, 5), (8, 64, 4), (11, 16, 16), (13, 32, 8), (16, 32, 8), (19, 0, 8)]:
-            bb.lib().b200_set_tuning(C.c_uint(c), C.c_uint(k1), C.c_uint(kn))
+            bb.set_tuning(c, k1, kn)
             assert np.array_equal(bb.compute_pedersen_commitments(0, cols, gens), want), (c, k1, kn)
     finally:
-        bb.lib().b200_set_tuning(C.c_uint(0), C.c_uint(0), C.c_uint(0))
+        bb.set_tuning()
 
 
 def test_homomorphism_through_partials(bb, port):
@@ -116,10 +115,8 @@ def test_homomorphism_through_partials(bb, port):
     pb = 128
     parts = bb.DeviceBuffer(2 * pb)
     bb.commit_device(0, [(n, 8, 0)] * 2, [ds[0].ptr, ds[1].ptr], dg.ptr, None, parts.ptr)
-    import ctypes as C
     out = bb.DeviceBuffer(32)
-    bb.lib().b200_combine_partials_device(C.c_uint(0), C.c_void_p(out.ptr), C.c_void_p(parts.ptr),
-                                          C.c_uint32(2), C.c_uint32(1))
+    bb.combine_partials_device(0, out.ptr, parts.ptr, 2, 1)
     want = bb.compute_pedersen_commitments(0, cols[2:], gens)
     assert np.array_equal(out.to_host()[:32], want[0])
 
@@ -170,7 +167,6 @@ def test_full_size_properties_c2(bb, port):
     """BASELINE config 2 size (ristretto, n = 2^20, 252-bit scalars): size-independent checks.
     (1) linearity: MSM over [0,n) == sum of the MSMs over two halves (partials + combine);
     (2) a 2^16 prefix with the remaining scalars zeroed equals the oracle on that prefix."""
-    import ctypes as C
     n = 1 << 20
     rng = np.random.default_rng(2)
     s = rng.integers(0, 256, (n, 32), dtype=np.uint8)
@@ -185,8 +181,7 @@ def test_full_size_properties_c2(bb, port):
     bb.commit_device(0, [(half, 32, 0)], [ds.ptr + half * 32], dg.ptr + half * 160, None,
                      parts.ptr + 128)
     out = bb.DeviceBuffer(32)
-    bb.lib().b200_combine_partials_device(C.c_uint(0), C.c_void_p(out.ptr), C.c_void_p(parts.ptr),
-                                          C.c_uint32(2), C.c_uint32(1))
+    bb.combine_partials_device(0, out.ptr, parts.ptr, 2, 1)
     assert np.array_equal(out.to_host()[:32], full[0])
     m = 1 << 14
     z = s.copy()
@@ -243,82 +238,70 @@ def test_default_piece_count_large_n(bb):
     assert np.array_equal(got, one)
 
 
-_MULTI_DEVICE_SCRIPT = r"""
-import sys, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200.api as bb
-from oracle import port
-from tests import common
-port.build()
-assert bb.sxt_init(num_precomputed_generators=64) == 0
-rng = np.random.default_rng(77)
-for curve, n, shapes in ((0, 5000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-4999, 8, 0), (0, 4, 1)]),
-                         (1, 700, [(0, 32, 0), (0, 2, 0), (-3, 8, 1)]),
-                         (2, 900, [(0, 32, 0)] * 7), (3, 300, [(0, 16, 0), (0, 16, 1)])):
-    gens, _ = common.generators_for(port, curve, n)
-    cols = common.random_columns(rng, n, shapes)
-    got = bb.compute_pedersen_commitments(curve, cols, gens)
-    assert common.same(curve, got, port.commit(curve, cols, gens)), curve
-cols = common.random_columns(rng, 3000, [(0, 8, 0)] * 9)  # built-in generators on every device
-assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, 11), port.commit(0, cols, None, 11))
-# fewer columns than devices: the generator RANGE is split, partial points gathered on device 0
-for curve, n, shapes in ((0, 5003, [(0, 32, 0)]), (1, 1300, [(0, 32, 0), (-700, 16, 1)]),
-                         (2, 2100, [(-1, 32, 0)]), (3, 999, [(0, 8, 1)])):
-    gens, _ = common.generators_for(port, curve, n)
-    cols = common.random_columns(rng, n, shapes)
-    got = bb.compute_pedersen_commitments(curve, cols, gens)
-    assert common.same(curve, got, port.commit(curve, cols, gens)), ("range", curve)
-cols = common.random_columns(rng, 4000, [(0, 32, 0)])
-assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, 5), port.commit(0, cols, None, 5))
-# handles are sharded over the devices at construction; fixed / packed / vlen calls and the file
-import tempfile, os
-for curve in range(4):
-    m = 1100
-    _, gens_p = common.generators_for(port, curve, m)
-    h = bb.MultiexpHandle(curve, gens_p)
-    sc = rng.integers(0, 256, (m, 2 * 32), dtype=np.uint8)
-    a = h.fixed_multiexponentiation(32, 2, m, sc)
-    b = port.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
-    assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("fixed", curve)
-    a = h.fixed_multiexponentiation(32, 2, 300, sc[:300])  # fewer rows than generators
-    b = port.fixed_msm(curve, gens_p, 2, 300, sc[:300], element_num_bytes=32)
-    assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("fixed300", curve)
-    bt = [3, 1, 14, 64, 5, 200]
-    psc = rng.integers(0, 256, (m, (sum(bt) + 7) // 8), dtype=np.uint8)
-    lens = [1, 2, 17, 400, 900, m]
-    a = h.fixed_vlen_multiexponentiation(bt, lens, psc)
-    b = port.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt, output_lengths=lens)
-    assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("vlen", curve)
-    path = os.path.join(tempfile.mkdtemp(), "h.bin")
-    h.write_to_file(path)
-    h2 = bb.MultiexpHandle(curve, filename=path)
-    a2 = h2.fixed_vlen_multiexponentiation(bt, lens, psc)
-    assert common.same(curve, port.normalize(curve, a2), port.normalize(curve, b)), ("file", curve)
-    h.free(); h2.free()
-    h3 = bb.MultiexpHandle(curve, filename=os.path.join(sys.argv[1], "tests", "golden", f"ref_table_curve{curve}_w3.bin"))
-    g7 = np.load(os.path.join(sys.argv[1], "tests", "golden", f"fixed_curve{curve}.npz"))["generators_p"][:7]
-    s7 = rng.integers(0, 256, (7, 32), dtype=np.uint8)
-    assert common.same(curve, port.normalize(curve, h3.fixed_multiexponentiation(32, 1, 7, s7)),
-                       port.normalize(curve, port.fixed_msm(curve, g7, 1, 7, s7, element_num_bytes=32)))
-    h3.free()
-print("multi-device ok")
-"""
+def _fresh_columns_split_over_devices(bb, port):
+    """By column, by generator range and sharded handles, BLITZAR_B200_DEVICES=k."""
+    rng = np.random.default_rng(77)
+    for curve, n, shapes in ((0, 5000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-4999, 8, 0), (0, 4, 1)]),
+                             (1, 700, [(0, 32, 0), (0, 2, 0), (-3, 8, 1)]),
+                             (2, 900, [(0, 32, 0)] * 7), (3, 300, [(0, 16, 0), (0, 16, 1)])):
+        gens, _ = common.generators_for(port, curve, n)
+        cols = common.random_columns(rng, n, shapes)
+        got = bb.compute_pedersen_commitments(curve, cols, gens)
+        assert common.same(curve, got, port.commit(curve, cols, gens)), curve
+    cols = common.random_columns(rng, 3000, [(0, 8, 0)] * 9)  # built-in generators on every device
+    assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, 11), port.commit(0, cols, None, 11))
+    # fewer columns than devices: the generator RANGE is split, partial points gathered on device 0
+    for curve, n, shapes in ((0, 5003, [(0, 32, 0)]), (1, 1300, [(0, 32, 0), (-700, 16, 1)]),
+                             (2, 2100, [(-1, 32, 0)]), (3, 999, [(0, 8, 1)])):
+        gens, _ = common.generators_for(port, curve, n)
+        cols = common.random_columns(rng, n, shapes)
+        got = bb.compute_pedersen_commitments(curve, cols, gens)
+        assert common.same(curve, got, port.commit(curve, cols, gens)), ("range", curve)
+    cols = common.random_columns(rng, 4000, [(0, 32, 0)])
+    assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, 5), port.commit(0, cols, None, 5))
+    # handles are sharded over the devices at construction; fixed / packed / vlen calls and the file
+    for curve in range(4):
+        m = 1100
+        _, gens_p = common.generators_for(port, curve, m)
+        h = bb.MultiexpHandle(curve, gens_p)
+        sc = rng.integers(0, 256, (m, 2 * 32), dtype=np.uint8)
+        a = h.fixed_multiexponentiation(32, 2, m, sc)
+        b = port.fixed_msm(curve, gens_p, 2, m, sc, element_num_bytes=32)
+        assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("fixed", curve)
+        a = h.fixed_multiexponentiation(32, 2, 300, sc[:300])  # fewer rows than generators
+        b = port.fixed_msm(curve, gens_p, 2, 300, sc[:300], element_num_bytes=32)
+        assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("fixed300", curve)
+        bt = [3, 1, 14, 64, 5, 200]
+        psc = rng.integers(0, 256, (m, (sum(bt) + 7) // 8), dtype=np.uint8)
+        lens = [1, 2, 17, 400, 900, m]
+        a = h.fixed_vlen_multiexponentiation(bt, lens, psc)
+        b = port.fixed_msm(curve, gens_p, len(bt), m, psc, output_bit_table=bt, output_lengths=lens)
+        assert common.same(curve, port.normalize(curve, a), port.normalize(curve, b)), ("vlen", curve)
+        path = os.path.join(tempfile.mkdtemp(), "h.bin")
+        h.write_to_file(path)
+        h2 = bb.MultiexpHandle(curve, filename=path)
+        a2 = h2.fixed_vlen_multiexponentiation(bt, lens, psc)
+        assert common.same(curve, port.normalize(curve, a2), port.normalize(curve, b)), ("file", curve)
+        h.free(); h2.free()
+        h3 = bb.MultiexpHandle(curve, filename=os.path.join(common.GOLDEN, f"ref_table_curve{curve}_w3.bin"))
+        g7 = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
+        s7 = rng.integers(0, 256, (7, 32), dtype=np.uint8)
+        assert common.same(curve, port.normalize(curve, h3.fixed_multiexponentiation(32, 1, 7, s7)),
+                           port.normalize(curve, port.fixed_msm(curve, g7, 1, 7, s7, element_num_bytes=32)))
+        h3.free()
 
 
-def test_columns_split_over_devices(bb):
+def test_columns_split_over_devices():
     """BLITZAR_B200_DEVICES=k: independent columns run on k devices of this process (the reference
     splits by output the same way, sxt/multiexp/pippenger2/multiexponentiation.h:248-287). With one
-    GPU, the test hook BLITZAR_B200_SHARED_DEVICES puts two shards on it."""
-    import subprocess
-    import sys
+    GPU, the test hook BLITZAR_B200_SHARED_DEVICES puts two shards on it. The same child runs the
+    per-column offsets entry point (tests/test_gpu_commit_offsets.py)."""
     import torch
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, BLITZAR_B200_DEVICES=str(max(2, min(4, torch.cuda.device_count()))),
+    env = dict(BLITZAR_B200_DEVICES=str(max(2, min(4, torch.cuda.device_count()))),
                BLITZAR_B200_SHARED_DEVICES="1" if torch.cuda.device_count() < 2 else "0",
                BLITZAR_B200_MIN_SHARD_TERMS="200")
-    r = subprocess.run([sys.executable, "-c", _MULTI_DEVICE_SCRIPT, root], env=env, cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "multi-device ok" in r.stdout, r.stdout + r.stderr
+    common.run_fresh(_fresh_columns_split_over_devices,
+                     test_gpu_commit_offsets._fresh_split_over_devices, env=env)
 
 
 # ---- fixed-base tables --------------------------------------------------------------------------------
@@ -356,8 +339,8 @@ def test_fixed_base_table_policies_agree(bb, port, curve, monkeypatch):
 def test_handle_from_reference_partition_table_file(bb, port, curve):
     """sxt_multiexp_handle_new_from_file reads the reference's own [u32 w][partition table] files
     (fixture written by the reference's code, tests/golden/make_table_files.py)."""
-    gens_p = np.load(os.path.join(GOLDEN_DIR, f"fixed_curve{curve}.npz"))["generators_p"][:7]
-    h = bb.MultiexpHandle(curve, filename=os.path.join(GOLDEN_DIR, f"ref_table_curve{curve}_w3.bin"))
+    gens_p = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
+    h = bb.MultiexpHandle(curve, filename=os.path.join(common.GOLDEN, f"ref_table_curve{curve}_w3.bin"))
     rng = np.random.default_rng(curve)
     sc = rng.integers(0, 256, (7, 32), dtype=np.uint8)
     got = h.fixed_multiexponentiation(32, 1, 7, sc)
@@ -366,34 +349,25 @@ def test_handle_from_reference_partition_table_file(bb, port, curve):
     h.free()
 
 
-def test_builtin_generator_table_subprocess():
+def _fresh_builtin_generator_table(bb, port):
+    rng = np.random.default_rng(3)
+    cols = common.random_columns(rng, 4000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-3999, 8, 0)])
+    for policy in ("1", "2", "0"):
+        os.environ["BLITZAR_B200_TABLE_POLICY"] = policy
+        for off in (0, 37, 1000, 4000):
+            assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, off),
+                                  port.commit(0, cols, None, off)), (policy, off)
+    g = bb.get_generators(10, 4995)
+    assert np.array_equal(port.normalize(0, g), port.normalize(0, port.ristretto_generators(10, 4995)))
+
+
+def test_builtin_generator_table():
     """num_precomputed_generators large enough for a fixed-base table over the built-in generators:
-    commitments inside, straddling and beyond it, table forced on / off / cost model."""
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    script = r'''
-import sys, os, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200.api as bb
-from oracle import port
-from tests import common
-port.build()
-assert bb.sxt_init(num_precomputed_generators=5000) == 0
-rng = np.random.default_rng(3)
-cols = common.random_columns(rng, 4000, [(0, 32, 0), (-100, 16, 1), (0, 1, 0), (-3999, 8, 0)])
-for policy in ("1", "2", "0"):
-    os.environ["BLITZAR_B200_TABLE_POLICY"] = policy
-    for off in (0, 37, 1000, 4000):
-        assert np.array_equal(bb.compute_pedersen_commitments(0, cols, None, off),
-                              port.commit(0, cols, None, off)), (policy, off)
-g = bb.get_generators(10, 4995)
-assert np.array_equal(port.normalize(0, g), port.normalize(0, port.ristretto_generators(10, 4995)))
-print("builtin table ok")
-'''
-    r = subprocess.run([sys.executable, "-c", script, root], cwd=root, capture_output=True, text=True,
-                       timeout=600)
-    assert r.returncode == 0 and "builtin table ok" in r.stdout, r.stdout + r.stderr
+    commitments inside, straddling and beyond it, table forced on / off / cost model; the same child
+    runs the per-column offsets entry point (tests/test_gpu_commit_offsets.py)."""
+    common.run_fresh(_fresh_builtin_generator_table,
+                     test_gpu_commit_offsets._fresh_builtin_generator_table,
+                     init={"num_precomputed_generators": 5000})
 
 
 def test_lane_sliced_field_arithmetic_selftest(bb):

@@ -4,10 +4,7 @@ degenerate input; the device entry with results and with partial points; handles
 reference's files and from files this library wrote; tables attached at construction by
 BLITZAR_B200_PARTITION_HANDLES; sharded handles; a Proof-of-SQL-like shape; and a table that does
 not fit."""
-import ctypes as C
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -16,8 +13,6 @@ from tests import common
 from tests import partition_tables as pt
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 WIDTHS = [1, 1, 1, 5, 1, 64, 256, 1, 13, 8, 1, 2]
 
 
@@ -80,14 +75,6 @@ def test_degenerate_generators_and_scalars(bb, port, curve, monkeypatch):
     h.free()
 
 
-def _device_call(bb, h, out_res, out_partials, mode, bt, lens, n, sc):
-    m = len(bt)
-    bb.lib().b200_fixed_msm_device(
-        C.c_void_p(out_res), C.c_void_p(out_partials), C.c_void_p(h.h), C.c_int(mode), C.c_uint(0),
-        (C.c_uint * m)(*bt), (C.c_uint * m)(*lens) if lens else None, C.c_uint(m), C.c_uint(n),
-        C.c_void_p(sc))
-
-
 @pytest.mark.parametrize("curve", [0, 2])
 def test_device_entry_results_and_partials(bb, port, curve, monkeypatch):
     n, w = 777, 5
@@ -105,10 +92,10 @@ def test_device_entry_results_and_partials(bb, port, curve, monkeypatch):
         for lens in (None, _lengths(n, w)):
             want = port.normalize(curve, port.fixed_msm(curve, gens, m, n, psc, output_bit_table=WIDTHS,
                                                         output_lengths=lens))
-            _device_call(bb, h, res.ptr, None, 2 if lens else 1, WIDTHS, lens, n, sc.ptr)
+            bb.fixed_msm_device(h, res.ptr, None, 0, m, n, sc.ptr, bit_table=WIDTHS, lengths=lens)
             got = res.to_host().reshape(m, proj)
             assert common.same(curve, port.normalize(curve, got), want), (policy, lens)
-            _device_call(bb, h, None, parts.ptr, 2 if lens else 1, WIDTHS, lens, n, sc.ptr)
+            bb.fixed_msm_device(h, None, parts.ptr, 0, m, n, sc.ptr, bit_table=WIDTHS, lengths=lens)
             bb.combine_partials_projective_device(curve, combined.ptr, parts.ptr, 1, m)
             got = combined.to_host().reshape(m, proj)
             assert common.same(curve, port.normalize(curve, got), want), (policy, lens)
@@ -122,8 +109,8 @@ def test_handles_from_files(bb, port, curve, tmp_path, monkeypatch):
     """The reference's own w = 3 file, and a w = 7 file this library wrote, read into handles that
     then carry partition tables."""
     monkeypatch.setenv("BLITZAR_B200_PARTITION_POLICY", "1")
-    g7 = np.load(os.path.join(GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
-    h = bb.MultiexpHandle(curve, filename=os.path.join(GOLDEN, f"ref_table_curve{curve}_w3.bin"))
+    g7 = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
+    h = bb.MultiexpHandle(curve, filename=os.path.join(common.GOLDEN, f"ref_table_curve{curve}_w3.bin"))
     assert h.add_partition_table(3) == 3
     _check_calls(port, curve, g7, h, np.random.default_rng(1), 7, 3)
     h.free()
@@ -139,60 +126,56 @@ def test_handles_from_files(bb, port, curve, tmp_path, monkeypatch):
     h.free()
 
 
-_SUBPROCESS = r"""
-import sys, os, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200 as bb
-from oracle import port
-from tests import common
-port.build()
-assert bb.sxt_init() == 0
-mode, out_dir = sys.argv[2], sys.argv[3]
-for curve in range(4):
-    n = 1100
-    _, gens = common.generators_for(port, curve, n, seed=17)
-    h = bb.MultiexpHandle(curve, gens)
-    if mode == "env":
+def _check_handles(bb, port, check_handle):
+    """Per curve, a handle over 1100 generators: check_handle(curve, h), then a vlen call whose lengths
+    straddle 550 (the shard boundary of two shards) against the oracle."""
+    for curve in range(4):
+        n = 1100
+        _, gens = common.generators_for(port, curve, n, seed=17)
+        h = bb.MultiexpHandle(curve, gens)
+        check_handle(curve, h)
+        bt = [1, 3, 64, 256, 1, 8]
+        psc = np.random.default_rng(curve).integers(0, 256, (n, (sum(bt) + 7) // 8), dtype=np.uint8)
+        lens = [0, 1, 549, 550, 551, n]
+        got = h.fixed_vlen_multiexponentiation(bt, lens, psc)
+        want = port.fixed_msm(curve, gens, len(bt), n, psc, output_bit_table=bt, output_lengths=lens)
+        assert common.same(curve, port.normalize(curve, got), port.normalize(curve, want)), curve
+        h.free()
+
+
+def test_tables_attached_at_construction(bb, port, tmp_path, monkeypatch):
+    """BLITZAR_B200_PARTITION_HANDLES=1: sxt_multiexp_handle_new and _new_from_file (both file
+    formats) attach a table at the default width (here BLITZAR_PARTITION_WINDOW_WIDTH=5)."""
+    monkeypatch.setenv("BLITZAR_B200_PARTITION_HANDLES", "1")
+    monkeypatch.setenv("BLITZAR_PARTITION_WINDOW_WIDTH", "5")
+    monkeypatch.setenv("BLITZAR_B200_PARTITION_POLICY", "1")
+
+    def attached_at_width_5(curve, h):
         assert h.partition_window == 5, h.partition_window
-        a, b = os.path.join(out_dir, f"{curve}.b2hd"), os.path.join(out_dir, f"{curve}.ref")
+        a, b = str(tmp_path / f"{curve}.b2hd"), str(tmp_path / f"{curve}.ref")
         h.write_to_file(a)
         h.write_partition_table(b, 7)
         for path in (a, b):
             h2 = bb.MultiexpHandle(curve, filename=path)
             assert h2.partition_window == 5, (path, h2.partition_window)
             h2.free()
-    else:
+
+    _check_handles(bb, port, attached_at_width_5)
+
+
+def _fresh_sharded_handles(bb, port):
+    def add_width_7(curve, h):
         assert h.add_partition_table(7) == 7 and h.partition_window == 7
-    bt = [1, 3, 64, 256, 1, 8]
-    psc = np.random.default_rng(curve).integers(0, 256, (n, (sum(bt) + 7) // 8), dtype=np.uint8)
-    lens = [0, 1, 549, 550, 551, n]
-    got = h.fixed_vlen_multiexponentiation(bt, lens, psc)
-    want = port.fixed_msm(curve, gens, len(bt), n, psc, output_bit_table=bt, output_lengths=lens)
-    assert common.same(curve, port.normalize(curve, got), port.normalize(curve, want)), curve
-    h.free()
-print("checked")
-"""
+
+    _check_handles(bb, port, add_width_7)
 
 
-def _run(mode, tmp_path, **env):
-    r = subprocess.run([sys.executable, "-c", _SUBPROCESS, ROOT, mode, str(tmp_path)],
-                       env=dict(os.environ, **env), cwd=ROOT, capture_output=True, text=True,
-                       timeout=900)
-    assert r.returncode == 0 and "checked" in r.stdout, r.stdout + r.stderr
-
-
-def test_tables_attached_at_construction(tmp_path):
-    """BLITZAR_B200_PARTITION_HANDLES=1: sxt_multiexp_handle_new and _new_from_file (both file
-    formats) attach a table at the default width (here BLITZAR_PARTITION_WINDOW_WIDTH=5)."""
-    _run("env", tmp_path, BLITZAR_B200_PARTITION_HANDLES="1", BLITZAR_PARTITION_WINDOW_WIDTH="5",
-         BLITZAR_B200_PARTITION_POLICY="1")
-
-
-def test_sharded_handles(tmp_path):
+def test_sharded_handles():
     """Two shards sharing the GPU, each with the table of its own generators: the shard boundary
     (550) is not a multiple of w = 7."""
-    _run("add", tmp_path, BLITZAR_B200_DEVICES="2", BLITZAR_B200_SHARED_DEVICES="1",
-         BLITZAR_B200_MIN_SHARD_TERMS="200", BLITZAR_B200_PARTITION_POLICY="1")
+    common.run_fresh(_fresh_sharded_handles,
+                     env=dict(BLITZAR_B200_DEVICES="2", BLITZAR_B200_SHARED_DEVICES="1",
+                              BLITZAR_B200_MIN_SHARD_TERMS="200", BLITZAR_B200_PARTITION_POLICY="1"))
 
 
 @pytest.mark.parametrize("curve", [0, 2])

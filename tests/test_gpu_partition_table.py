@@ -4,8 +4,6 @@ b200_multiexp_handle_write_partition_table): the fixtures written by the referen
 grumpkin and value for value on ristretto255, the files read back into handles, many chunks, sharded
 handles, the default window width, and a full-size table checked entry by entry against the oracle."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -14,16 +12,14 @@ from tests import common
 from tests import partition_tables as pt
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def fixture_cases(curve):
     """(name, projective generators, window width, reference digest of the table)."""
-    g7 = np.load(os.path.join(GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
-    ref = np.fromfile(os.path.join(GOLDEN, f"ref_table_curve{curve}_w3.bin"), dtype=np.uint8)
+    g7 = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
+    ref = np.fromfile(os.path.join(common.GOLDEN, f"ref_table_curve{curve}_w3.bin"), dtype=np.uint8)
     out = [("n7_w3", g7, 3, pt.table_digest(curve, ref[4:]))]
-    z = np.load(os.path.join(GOLDEN, f"ptable_curve{curve}.npz"))
+    z = np.load(os.path.join(common.GOLDEN, f"ptable_curve{curve}.npz"))
     for name, (_, w, _) in pt.CASES.items():
         out.append((name, z[f"gens_{name}"], w, str(z[f"sha_{name}"])))
     return out
@@ -117,35 +113,21 @@ def test_many_chunks_give_the_same_file(bb, port, curve, tmp_path, monkeypatch):
     assert files[0][4:] == tables[0].tobytes()
 
 
-_SUBPROCESS = r"""
-import sys, os, numpy as np
-sys.path.insert(0, sys.argv[1])
-import blitzar_b200 as bb
-from oracle import port
-from tests import common
-port.build()
-assert bb.sxt_init() == 0
-for curve in range(4):
-    _, gens_p = common.generators_for(port, curve, 1100)
-    h = bb.MultiexpHandle(curve, gens_p)
-    h.write_partition_table(os.path.join(sys.argv[2], f"{curve}.bin"), int(sys.argv[3]))
-    h.free()
-print("written")
-"""
-
-
-def _write_in_subprocess(out_dir, window_width, **env):
-    r = subprocess.run([sys.executable, "-c", _SUBPROCESS, ROOT, str(out_dir), str(window_width)],
-                       env=dict(os.environ, **env), cwd=ROOT, capture_output=True, text=True,
-                       timeout=900)
-    assert r.returncode == 0 and "written" in r.stdout, r.stdout + r.stderr
+def _write_tables(bb, port, out_dir, window_width):
+    """out_dir/{curve}.bin: the file of 1100 generators per curve at window_width."""
+    for curve in range(4):
+        _, gens_p = common.generators_for(port, curve, 1100)
+        h = bb.MultiexpHandle(curve, gens_p)
+        h.write_partition_table(os.path.join(out_dir, f"{curve}.bin"), window_width)
+        h.free()
 
 
 def test_sharded_handles_write_the_same_file(bb, port, tmp_path):
     """BLITZAR_B200_DEVICES=2 (two shards sharing the GPU): the shards' generators are gathered in
     order; the shard boundary (550) is not a multiple of w = 7."""
-    _write_in_subprocess(tmp_path, 7, BLITZAR_B200_DEVICES="2", BLITZAR_B200_SHARED_DEVICES="1",
-                         BLITZAR_B200_MIN_SHARD_TERMS="200")
+    common.run_fresh((_write_tables, str(tmp_path), 7),
+                     env=dict(BLITZAR_B200_DEVICES="2", BLITZAR_B200_SHARED_DEVICES="1",
+                              BLITZAR_B200_MIN_SHARD_TERMS="200"))
     for curve in range(4):
         _, gens_p = common.generators_for(port, curve, 1100)
         h = bb.MultiexpHandle(curve, gens_p)
@@ -155,7 +137,7 @@ def test_sharded_handles_write_the_same_file(bb, port, tmp_path):
         assert open(path, "rb").read() == open(tmp_path / f"{curve}.bin", "rb").read(), curve
 
 
-def test_default_window_width(bb, port, tmp_path):
+def test_default_window_width(bb, port, tmp_path, monkeypatch):
     """window_width 0: 16, or BLITZAR_PARTITION_WINDOW_WIDTH as the reference reads it."""
     _, gens_p = common.generators_for(port, 2, 40)
     h = bb.MultiexpHandle(2, gens_p)
@@ -164,7 +146,8 @@ def test_default_window_width(bb, port, tmp_path):
     h.free()
     w, table = read_file(path)
     assert w == 16 and table.size == bb.partition_table_bytes(2, 40, 16)
-    _write_in_subprocess(tmp_path, 0, BLITZAR_PARTITION_WINDOW_WIDTH="5")
+    monkeypatch.setenv("BLITZAR_PARTITION_WINDOW_WIDTH", "5")
+    _write_tables(bb, port, str(tmp_path), 0)
     for curve in range(4):
         w, table = read_file(str(tmp_path / f"{curve}.bin"))
         assert w == 5 and table.size == bb.partition_table_bytes(curve, 1100, 5), curve

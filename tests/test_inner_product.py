@@ -8,12 +8,13 @@ import os
 import numpy as np
 import pytest
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "inner_product.npz")
-L = 2**252 + 27742317777372353535851937790883648493
+from tests import common
+
+L =2**252 + 27742317777372353535851937790883648493
 
 
 def _check_against_fixture(engine):
-    z = np.load(GOLDEN)
+    z = np.load(os.path.join(common.GOLDEN, "inner_product.npz"))
     off = int(z["generators_offset"])
     for ci in range(int(z["num_cases"])):
         a, b = z[f"a{ci}"], z[f"b{ci}"]

@@ -6,8 +6,6 @@ import numpy as np
 
 from tests import common
 
-GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
 
 def test_port_reproduces_reference_golden_commitments(port):
     out = port.commit(0, common.golden_columns())
@@ -16,11 +14,11 @@ def test_port_reproduces_reference_golden_commitments(port):
 
 def test_port_matches_committed_reference_fixtures(port):
     for curve in range(4):
-        z = np.load(os.path.join(GOLDEN_DIR, f"commit_curve{curve}.npz"))
+        z = np.load(os.path.join(common.GOLDEN, f"commit_curve{curve}.npz"))
         cols = [(z[f"col{j}"], int(z["signed"][j])) for j in range(len(z["signed"]))]
         out = port.commit(curve, cols, z["generators"])
         assert common.same(curve, out, z["commitments"]), curve
-        f = np.load(os.path.join(GOLDEN_DIR, f"fixed_curve{curve}.npz"))
+        f = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))
         res = port.fixed_msm(curve, f["generators_p"], int(f["num_outputs"]), int(f["n"]),
                              f["scalars"], element_num_bytes=int(f["element_num_bytes"]))
         assert common.same(curve, port.normalize(curve, res), f["normalized"]), curve
@@ -30,7 +28,7 @@ def test_port_matches_committed_reference_fixtures(port):
 
 
 def test_builtin_generators_fixture(port):
-    z = np.load(os.path.join(GOLDEN_DIR, "ristretto_generators.npz"))
+    z = np.load(os.path.join(common.GOLDEN, "ristretto_generators.npz"))
     g = port.ristretto_generators(int(z["n"]), int(z["offset"]))
     assert np.array_equal(port.normalize(0, g), z["compressed"])
 

@@ -7,15 +7,14 @@ import os
 import numpy as np
 import pytest
 
+from tests import common
 from tests import partition_tables as pt
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
 def test_reference_w3_file_is_reproduced(emul, curve):
-    g7 = np.load(os.path.join(GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
-    ref = np.fromfile(os.path.join(GOLDEN, f"ref_table_curve{curve}_w3.bin"), dtype=np.uint8)
+    g7 = np.load(os.path.join(common.GOLDEN, f"fixed_curve{curve}.npz"))["generators_p"][:7]
+    ref = np.fromfile(os.path.join(common.GOLDEN, f"ref_table_curve{curve}_w3.bin"), dtype=np.uint8)
     assert int(ref[:4].view("<u4")[0]) == 3
     got = emul.partition_table(curve, g7, 3)
     want = pt.canonicalise_ristretto_table(ref[4:]) if curve == 0 else ref[4:]
@@ -26,7 +25,7 @@ def test_reference_w3_file_is_reproduced(emul, curve):
 @pytest.mark.parametrize("curve", [0, 1, 2, 3])
 @pytest.mark.parametrize("case", list(pt.CASES))
 def test_fixture_digests(emul, curve, case):
-    z = np.load(os.path.join(GOLDEN, f"ptable_curve{curve}.npz"))
+    z = np.load(os.path.join(common.GOLDEN, f"ptable_curve{curve}.npz"))
     gens = z[f"gens_{case}"]
     _, w, _ = pt.CASES[case]
     got = emul.partition_table(curve, gens, w)
@@ -41,7 +40,7 @@ def test_fixture_digests(emul, curve, case):
 def test_generators_read_back(emul, port, curve, tmp_path):
     """Entry 1 << j of group g is generator g w + j: the reader of reference handle files recovers
     the generators (the padding of the last group reads back as the identity)."""
-    z = np.load(os.path.join(GOLDEN, f"ptable_curve{curve}.npz"))
+    z = np.load(os.path.join(common.GOLDEN, f"ptable_curve{curve}.npz"))
     for case in ("n37_w8", "n24_w6_edited"):
         gens = z[f"gens_{case}"]
         _, w, _ = pt.CASES[case]

@@ -9,8 +9,6 @@ import pytest
 
 from tests import common
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 def test_shard_ranges_cover_and_balance():
     from blitzar_b200.sharding import shard_range
@@ -32,7 +30,7 @@ def _free_port():
 
 
 def _worker(rank, world_size, port_no, curve, out_queue):
-    sys.path.insert(0, ROOT)
+    sys.path.insert(0, common.ROOT)
     import torch
     import torch.distributed as dist
     from blitzar_b200.sharding import sharded_commit
