@@ -44,6 +44,7 @@ B200_SYMBOLS = [
     "b200_multiexp_handle_write_partition_table",
     "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
     "b200_multiexp_handle_add_partition_table", "b200_multiexp_handle_partition_window",
+    "b200_curve25519_prove_inner_products", "b200_curve25519_verify_inner_products",
 ]
 
 
@@ -486,3 +487,74 @@ def verify_inner_product(transcript, b, product, a_commit, l_vector, r_vector, a
         _ptr(transcript), C.c_uint64(n), C.c_uint64(generators_offset), _ptr(b),
         _ptr(np.ascontiguousarray(product)), _ptr(np.ascontiguousarray(a_commit)), _ptr(lv),
         _ptr(rv), _ptr(np.ascontiguousarray(ap_value))))
+
+
+def _ipa_batch_inputs(vectors, offsets):
+    """(n uint64 [P], offsets uint64 [P], concatenated uint8 [sum n, 32], round counts)."""
+    n = np.array([v.shape[0] for v in vectors], dtype=np.uint64)
+    offs = np.zeros(len(vectors), np.uint64) if offsets is None else \
+        np.ascontiguousarray(offsets, dtype=np.uint64)
+    if offs.shape != n.shape:
+        raise ValueError("one generators offset per proof")
+    flat = np.ascontiguousarray(np.concatenate([np.asarray(v, np.uint8).reshape(-1, 32)
+                                                for v in vectors])) if len(vectors) else \
+        np.zeros((1, 32), np.uint8)
+    rounds = [max(0, (int(m) - 1).bit_length()) for m in n]
+    return n, offs, flat, rounds
+
+
+def prove_inner_products(transcripts, a_list, b_list, offsets=None):
+    """b200_curve25519_prove_inner_products. transcripts: uint8 [P, 203] (advanced in place);
+    a_list, b_list: P arrays of uint8 [n_p, 32]; offsets: P generator offsets (None = all 0).
+    Returns [(l_vector [k_p, 32], r_vector, ap_value [32])] per proof, as prove_inner_product."""
+    return call_prove_inner_products(lib().b200_curve25519_prove_inner_products, transcripts,
+                                     a_list, b_list, offsets)
+
+
+def verify_inner_products(transcripts, b_list, products, a_commits, l_list, r_list, ap_values,
+                          offsets=None):
+    """b200_curve25519_verify_inner_products -> int32 results [P] (1 / 0). transcripts: uint8
+    [P, 203] (advanced in place); b_list, l_list, r_list: P arrays of uint8 [n_p, 32] / [k_p, 32];
+    products, ap_values: uint8 [P, 32]; a_commits: uint8 [P, 160]."""
+    lib().b200_curve25519_verify_inner_products.restype = C.c_uint32
+    return call_verify_inner_products(lib().b200_curve25519_verify_inner_products, transcripts,
+                                      b_list, products, a_commits, l_list, r_list, ap_values,
+                                      offsets)
+
+
+def call_prove_inner_products(entry, transcripts, a_list, b_list, offsets=None):
+    """prove_inner_products through `entry`, a C function with the batch prover's arguments."""
+    if len(a_list) != len(b_list) or any(a.shape[0] != b.shape[0] for a, b in zip(a_list, b_list)):
+        raise ValueError("a_list and b_list must hold vectors of equal lengths")
+    if transcripts.shape != (len(a_list), 203) or not transcripts.flags.c_contiguous:
+        raise ValueError("transcripts must be a contiguous uint8 [P, 203] array")
+    n, offs, a, rounds = _ipa_batch_inputs(a_list, offsets)
+    _, _, b, _ = _ipa_batch_inputs(b_list, offsets)
+    nk = sum(rounds)
+    lv = np.zeros((max(nk, 1), 32), dtype=np.uint8)
+    rv = np.zeros((max(nk, 1), 32), dtype=np.uint8)
+    ap = np.zeros((max(len(a_list), 1), 32), dtype=np.uint8)
+    entry(C.c_uint32(len(a_list)), _ptr(lv), _ptr(rv), _ptr(ap), _ptr(transcripts), _ptr(n),
+          _ptr(offs), _ptr(a), _ptr(b))
+    out, k0 = [], 0
+    for p, k in enumerate(rounds):
+        out.append((lv[k0:k0 + k], rv[k0:k0 + k], ap[p]))
+        k0 += k
+    return out
+
+
+def call_verify_inner_products(entry, transcripts, b_list, products, a_commits, l_list, r_list,
+                               ap_values, offsets=None):
+    """verify_inner_products through `entry`, a C function with the batch verifier's arguments."""
+    P = len(b_list)
+    if transcripts.shape != (P, 203) or not transcripts.flags.c_contiguous:
+        raise ValueError("transcripts must be a contiguous uint8 [P, 203] array")
+    n, offs, b, _ = _ipa_batch_inputs(b_list, offsets)
+    lrs = [np.concatenate([np.asarray(v, np.uint8).reshape(-1, 32) for v in vs] +
+                          [np.zeros((1, 32), np.uint8)]) for vs in (l_list, r_list)]
+    results = np.zeros(max(P, 1), dtype=np.int32)
+    entry(C.c_uint32(P), _ptr(results), _ptr(transcripts), _ptr(n), _ptr(offs), _ptr(b),
+          _ptr(np.ascontiguousarray(products, np.uint8)),
+          _ptr(np.ascontiguousarray(a_commits, np.uint8)), _ptr(np.ascontiguousarray(lrs[0])),
+          _ptr(np.ascontiguousarray(lrs[1])), _ptr(np.ascontiguousarray(ap_values, np.uint8)))
+    return results[:P]

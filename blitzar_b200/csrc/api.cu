@@ -1045,6 +1045,79 @@ int sxt_curve25519_verify_inner_product(struct sxt_transcript* transcript, uint6
                     reinterpret_cast<const uint8_t*>(l_vector),
                     reinterpret_cast<const uint8_t*>(r_vector), ap_value->bytes);
 }
+// The batch calls check every proof as the single calls do, on the calling thread before any device
+// work, and that the batch's generator arena stays below the engine's 31-bit generator index
+// (prover: [G_p | Q_p] = np_p + 1 per proof; verifier: [Q_p, G_p, L_p, R_p] and a [Q_p, A_p] pair).
+namespace {
+unsigned ipa_rounds(uint64_t n) {
+  unsigned k = 0;
+  while ((1ull << k) < n)
+    ++k;
+  return k;
+}
+void check_ipa_batch(uint32_t num_proofs, const uint64_t* n, const uint64_t* generators_offsets,
+                     const void* transcripts, bool prover) {
+  B200_REQUIRE(transcripts != nullptr && n != nullptr && generators_offsets != nullptr,
+               "transcripts / n / generators_offsets must not be null");
+  uint64_t arena = 0;
+  for (uint32_t p = 0; p < num_proofs; ++p) {
+    B200_REQUIRE(n[p] > 0, "a_vector and b_vector lengths must be greater than zero");
+    B200_REQUIRE(n[p] < (1ull << 30), "n too large");
+    const unsigned k = ipa_rounds(n[p]);
+    arena += prover ? (1ull << k) + 1 : (1ull << k) + 2 * k + 3;
+  }
+  B200_REQUIRE(arena < (1ull << 31), "proofs of the batch need too many generators for one call");
+}
+bool any_rounds(uint32_t num_proofs, const uint64_t* n) {
+  for (uint32_t p = 0; p < num_proofs; ++p)
+    if (n[p] > 1)
+      return true;
+  return false;
+}
+}  // namespace
+
+void b200_curve25519_prove_inner_products(
+    uint32_t num_proofs, struct sxt_ristretto255_compressed* l_vectors,
+    struct sxt_ristretto255_compressed* r_vectors, struct sxt_curve25519_scalar* ap_values,
+    struct sxt_transcript* transcripts, const uint64_t* n, const uint64_t* generators_offsets,
+    const struct sxt_curve25519_scalar* a_vectors, const struct sxt_curve25519_scalar* b_vectors) {
+  const Entry entry("b200_curve25519_prove_inner_products");
+  if (num_proofs == 0)
+    return;
+  check_ipa_batch(num_proofs, n, generators_offsets, transcripts, true);
+  B200_REQUIRE(ap_values != nullptr, "ap_values must not be null");
+  B200_REQUIRE(b_vectors != nullptr && a_vectors != nullptr, "a_vectors / b_vectors must not be null");
+  B200_REQUIRE(!any_rounds(num_proofs, n) || (l_vectors != nullptr && r_vectors != nullptr),
+               "l_vectors and r_vectors must not be null when some n > 1");
+  ipa_prove_batch(ctx(), num_proofs, reinterpret_cast<uint8_t*>(l_vectors),
+                  reinterpret_cast<uint8_t*>(r_vectors), ap_values->bytes, transcripts->bytes, n,
+                  generators_offsets, reinterpret_cast<const uint8_t*>(a_vectors),
+                  reinterpret_cast<const uint8_t*>(b_vectors));
+}
+uint32_t b200_curve25519_verify_inner_products(
+    uint32_t num_proofs, int* results, struct sxt_transcript* transcripts, const uint64_t* n,
+    const uint64_t* generators_offsets, const struct sxt_curve25519_scalar* b_vectors,
+    const struct sxt_curve25519_scalar* products, const struct sxt_ristretto255* a_commits,
+    const struct sxt_ristretto255_compressed* l_vectors,
+    const struct sxt_ristretto255_compressed* r_vectors,
+    const struct sxt_curve25519_scalar* ap_values) {
+  const Entry entry("b200_curve25519_verify_inner_products");
+  if (num_proofs == 0)
+    return 0;
+  check_ipa_batch(num_proofs, n, generators_offsets, transcripts, false);
+  B200_REQUIRE(results != nullptr, "results must not be null");
+  B200_REQUIRE(ap_values != nullptr && products != nullptr && a_commits != nullptr &&
+                   b_vectors != nullptr,
+               "ap_values / products / a_commits / b_vectors must not be null");
+  B200_REQUIRE(!any_rounds(num_proofs, n) || (l_vectors != nullptr && r_vectors != nullptr),
+               "l_vectors and r_vectors must not be null when some n > 1");
+  return ipa_verify_batch(ctx(), num_proofs, results, transcripts->bytes, n, generators_offsets,
+                          reinterpret_cast<const uint8_t*>(b_vectors), products->bytes,
+                          reinterpret_cast<const uint8_t*>(a_commits),
+                          reinterpret_cast<const uint8_t*>(l_vectors),
+                          reinterpret_cast<const uint8_t*>(r_vectors), ap_values->bytes);
+}
+
 void sxt_prove_sumcheck(void*, void*, unsigned, const struct sumcheck_descriptor*, void*, void*) {
   die("sxt_prove_sumcheck is not provided by blitzar_b200 (MSM hot path only)", __FILE__,
       __LINE__);

@@ -46,7 +46,25 @@ int ipa_verify(const EngineCtx& ctx, uint8_t* transcript203, uint64_t n,
                uint64_t generators_offset, const uint8_t* b_vector, const uint8_t* product,
                const uint8_t* a_commit160, const uint8_t* l_vector, const uint8_t* r_vector,
                const uint8_t* ap_value) {
-  return Ipa::verify(ctx, transcript203, n, generators_offset, b_vector, product, a_commit160,
-                     l_vector, r_vector, ap_value);
+  int result = 0;  // a batch of one
+  IpaBatch::verify(ctx, 1, &result, transcript203, &n, &generators_offset, b_vector, product,
+                   a_commit160, l_vector, r_vector, ap_value);
+  return result;
+}
+void ipa_prove_batch(const EngineCtx& ctx, uint32_t num_proofs, uint8_t* l_vectors,
+                     uint8_t* r_vectors, uint8_t* ap_values, uint8_t* transcripts,
+                     const uint64_t* n, const uint64_t* generators_offsets,
+                     const uint8_t* a_vectors, const uint8_t* b_vectors) {
+  IpaBatch::prove(ctx, num_proofs, l_vectors, r_vectors, ap_values, transcripts, n,
+                  generators_offsets, a_vectors, b_vectors);
+}
+uint32_t ipa_verify_batch(const EngineCtx& ctx, uint32_t num_proofs, int* results,
+                          uint8_t* transcripts, const uint64_t* n,
+                          const uint64_t* generators_offsets, const uint8_t* b_vectors,
+                          const uint8_t* products, const uint8_t* a_commits,
+                          const uint8_t* l_vectors, const uint8_t* r_vectors,
+                          const uint8_t* ap_values) {
+  return IpaBatch::verify(ctx, num_proofs, results, transcripts, n, generators_offsets, b_vectors,
+                          products, a_commits, l_vectors, r_vectors, ap_values);
 }
 }  // namespace b200

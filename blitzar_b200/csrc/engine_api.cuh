@@ -288,6 +288,7 @@ inline const CurveVTable& curve_vtable(unsigned curve_id) {
 }
 
 // inner-product argument over ristretto255 (ipa.cuh); same contracts as the two sxt_* entry points
+// (ipa_verify runs a batch of one) and as the two b200_* batch entry points (IpaBatch)
 void ipa_prove(const EngineCtx& ctx, uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value,
                uint8_t* transcript203, uint64_t n, uint64_t generators_offset,
                const uint8_t* a_vector, const uint8_t* b_vector);
@@ -295,6 +296,16 @@ int ipa_verify(const EngineCtx& ctx, uint8_t* transcript203, uint64_t n,
                uint64_t generators_offset, const uint8_t* b_vector, const uint8_t* product,
                const uint8_t* a_commit160, const uint8_t* l_vector, const uint8_t* r_vector,
                const uint8_t* ap_value);
+void ipa_prove_batch(const EngineCtx& ctx, uint32_t num_proofs, uint8_t* l_vectors,
+                     uint8_t* r_vectors, uint8_t* ap_values, uint8_t* transcripts,
+                     const uint64_t* n, const uint64_t* generators_offsets,
+                     const uint8_t* a_vectors, const uint8_t* b_vectors);
+uint32_t ipa_verify_batch(const EngineCtx& ctx, uint32_t num_proofs, int* results,
+                          uint8_t* transcripts, const uint64_t* n,
+                          const uint64_t* generators_offsets, const uint8_t* b_vectors,
+                          const uint8_t* products, const uint8_t* a_commits,
+                          const uint8_t* l_vectors, const uint8_t* r_vectors,
+                          const uint8_t* ap_values);
 
 // lane-sliced field arithmetic self-test (lanefield.cuh): number of mismatching checks over
 // `warps` warps of pseudo-random / edge-case operands

@@ -257,6 +257,30 @@ unsigned b200_multiexp_handle_add_partition_table(struct sxt_multiexp_handle* ha
                                                   unsigned window_width);
 /* Width of the handle's partition table, or 0 when it has none. */
 unsigned b200_multiexp_handle_partition_window(const struct sxt_multiexp_handle* handle);
+/* Proves num_proofs independent inner-product arguments in one call. Proof p, and transcripts[p], are
+ * byte-identical to sxt_curve25519_prove_inner_product(l, r, &ap_values[p], &transcripts[p], n[p],
+ * generators_offsets[p], a_p, b_p) called alone. Arrays are flattened in proof order: with
+ * k_p = ceil(log2 n_p), proof p's L / R values start at the sum of k_q over the proofs q < p, its a / b
+ * scalars at the sum of n_q. Every round of every proof runs in one engine pass per round of the
+ * longest proof. Host pointers; synchronises. num_proofs == 0: no-op. */
+void b200_curve25519_prove_inner_products(
+    uint32_t num_proofs, struct sxt_ristretto255_compressed* l_vectors /* sum k_p */,
+    struct sxt_ristretto255_compressed* r_vectors /* sum k_p */,
+    struct sxt_curve25519_scalar* ap_values /* num_proofs */,
+    struct sxt_transcript* transcripts /* num_proofs, advanced in place */, const uint64_t* n,
+    const uint64_t* generators_offsets, const struct sxt_curve25519_scalar* a_vectors /* sum n_p */,
+    const struct sxt_curve25519_scalar* b_vectors /* sum n_p */);
+/* results[p] = what sxt_curve25519_verify_inner_product returns for proof p alone (1 / 0), transcripts
+ * advanced as that call advances them; arrays flattened as for b200_curve25519_prove_inner_products
+ * (products, a_commits, ap_values: one per proof). One engine pass for the whole batch. Returns the
+ * number of accepted proofs. Host pointers; synchronises. */
+uint32_t b200_curve25519_verify_inner_products(
+    uint32_t num_proofs, int* results, struct sxt_transcript* transcripts, const uint64_t* n,
+    const uint64_t* generators_offsets, const struct sxt_curve25519_scalar* b_vectors /* sum n_p */,
+    const struct sxt_curve25519_scalar* products, const struct sxt_ristretto255* a_commits,
+    const struct sxt_ristretto255_compressed* l_vectors /* sum k_p */,
+    const struct sxt_ristretto255_compressed* r_vectors /* sum k_p */,
+    const struct sxt_curve25519_scalar* ap_values);
 /* Self-test of the warp-cooperative (lane-sliced) field arithmetic of the tail kernels against the
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
