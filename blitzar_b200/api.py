@@ -40,7 +40,8 @@ B200_SYMBOLS = [
     "b200_profile_read", "b200_set_reduce_groups", "b200_stream",
     "b200_synthetic_generators_device", "b200_commit_host_partials",
     "b200_fixed_msm_host_partials", "b200_multiexp_handle_new_device",
-    "b200_selftest_lane_arithmetic", "b200_selftest_sort", "b200_partition_table_device",
+    "b200_selftest_lane_arithmetic", "b200_selftest_field_multiply", "b200_selftest_sort",
+    "b200_partition_table_device",
     "b200_multiexp_handle_write_partition_table",
     "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
     "b200_multiexp_handle_add_partition_table", "b200_multiexp_handle_partition_window",
@@ -334,6 +335,11 @@ def commit_device_with_offsets(curve_id, columns_shape, scalar_ptrs, generators_
 def selftest_lane_arithmetic(warps=64, seed=1):
     lib().b200_selftest_lane_arithmetic.restype = C.c_uint
     return int(lib().b200_selftest_lane_arithmetic(C.c_uint(warps), C.c_uint(seed)))
+
+
+def selftest_field_multiply(threads=1 << 16, seed=1):
+    lib().b200_selftest_field_multiply.restype = C.c_uint
+    return int(lib().b200_selftest_field_multiply(C.c_uint(threads), C.c_uint(seed)))
 
 
 def selftest_sort(columns_shape, scalar_ptrs, window_bits=0):

@@ -1486,6 +1486,10 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   const Entry entry("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);
 }
+unsigned b200_selftest_field_multiply(unsigned threads, unsigned seed) {
+  const Entry entry("b200_selftest_field_multiply");
+  return selftest_field_multiply(ctx(), threads, seed);
+}
 unsigned b200_selftest_sort(const sxt_sequence_descriptor* columns, unsigned num,
                             unsigned window_bits) {
   const Entry entry("b200_selftest_sort");

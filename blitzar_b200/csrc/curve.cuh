@@ -204,24 +204,26 @@ struct Ed25519 {
   template <class X = SeqExec>
   static B200_HD void add_gen(Point& r, const Point& a, const Gen& g, bool negate,
                               bool unit_z = false) {
-    fe A, B, C, D, E, Fv, G, H, t0, t1, qp, qm, qt, nt;
+    // -g negates C = T1 2dT2, which swaps D - C and D + C: selected after the sums rather than
+    // negating 2dT2 before the product
+    fe A, B, C, D, E, Fv, G, H, t0, t1, qp, qm, dmc, dpc;
     F::select(qp, g.YpX, g.YmX, negate);
     F::select(qm, g.YmX, g.YpX, negate);
-    F::neg(nt, g.T2d);
-    F::select(qt, g.T2d, nt, negate);
     F::sub(t0, a.Y, a.X);
     F::add(t1, a.Y, a.X);
     if (unit_z) {
       F::mul(A, t0, qm);
       F::mul(B, t1, qp);
-      F::mul(C, a.T, qt);
+      F::mul(C, a.T, g.T2d);
       F::dbl(D, a.Z);
     } else {
-      X::template mul4<F>(A, B, C, D, t0, qm, t1, qp, a.T, qt, a.Z, g.Z2);
+      X::template mul4<F>(A, B, C, D, t0, qm, t1, qp, a.T, g.T2d, a.Z, g.Z2);
     }
     F::sub(E, B, A);
-    F::sub(Fv, D, C);
-    F::add(G, D, C);
+    F::sub(dmc, D, C);
+    F::add(dpc, D, C);
+    F::select(Fv, dmc, dpc, negate);
+    F::select(G, dpc, dmc, negate);
     F::add(H, B, A);
     Point o;
     X::template mul4<F>(o.X, o.Y, o.T, o.Z, E, Fv, G, H, E, H, Fv, G);

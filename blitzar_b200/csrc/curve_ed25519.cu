@@ -4,6 +4,67 @@
 #include "ipa.cuh"
 namespace b200 {
 B200_DEFINE_CURVE_VTABLE(kVTableEd25519, Ed25519);
+
+// Self-test body (b200_selftest_field_multiply): F25519::mul, the carry-chain schedule the kernels
+// run, against the plain 64-bit schedule F25519::mul_ref, limb for limb (both fold the same
+// 512-bit product to the same loosely reduced residue). Operand a of thread t is edge case t % 10,
+// b is edge case t / 10 % 10 (9 = random), so every pair of edge cases meets; beyond the first
+// 100 threads one limb of a or b is also forced to all ones.
+struct FieldMulSelfTestBody {
+  static constexpr int kBlock = 128;
+  u32 seed;
+  u32* mismatches;
+  static B200_HD u32 rnd(u64& st) {
+    st ^= st << 13;
+    st ^= st >> 7;
+    st ^= st << 17;
+    return (u32)(st >> 16);
+  }
+  static B200_HD void operand(F25519::E& x, u32 k, u64& st) {
+    for (int i = 0; i < 8; ++i)
+      x.l[i] = rnd(st);
+    const u32 ones = 0xffffffffu;
+    switch (k) {
+    case 0: for (int i = 0; i < 8; ++i) x.l[i] = 0; break;                                 // 0
+    case 1: for (int i = 0; i < 8; ++i) x.l[i] = i == 0; break;                            // 1
+    case 2: for (int i = 0; i < 8; ++i) x.l[i] = ones; x.l[0] = 0xffffffecu; x.l[7] >>= 1; break;  // p - 1
+    case 3: for (int i = 0; i < 8; ++i) x.l[i] = ones; x.l[0] = 0xffffffedu; x.l[7] >>= 1; break;  // p
+    case 4: for (int i = 0; i < 8; ++i) x.l[i] = ones; x.l[7] >>= 1; break;                // p + 18
+    case 5: for (int i = 0; i < 8; ++i) x.l[i] = 0; x.l[7] = 0x80000000u; break;           // 2^255
+    case 6: for (int i = 0; i < 8; ++i) x.l[i] = ones; break;                              // 2^256 - 1
+    case 7: for (int i = 0; i < 8; ++i) x.l[i] = ones; x.l[0] = 0xffffffdau; break;        // 2^256 - 38
+    case 8: for (int i = 0; i < 8; ++i) x.l[i] = i < 4 ? ones : 0u; break;                 // 2^128 - 1
+    default: break;
+    }
+  }
+  B200_HD void operator()(u64 tid) const {
+    u64 st = ((u64)seed << 32) ^ (0x9E3779B97F4A7C15ull * (tid + 1));
+    F25519::E a, b, got, want;
+    operand(a, (u32)(tid % 10), st);
+    operand(b, (u32)(tid / 10 % 10), st);
+    const u32 f = (u32)(tid / 100);
+    if (f % 3 == 1)
+      a.l[f / 3 % 8] = 0xffffffffu;
+    if (f % 3 == 2)
+      b.l[f / 3 % 8] = 0xffffffffu;
+    F25519::mul(got, a, b);
+    F25519::mul_ref(want, a, b);
+    u32 diff = 0;
+    for (int i = 0; i < 8; ++i)
+      diff |= got.l[i] ^ want.l[i];
+    if (diff)
+      B200_ATOMIC_ADD(mismatches, 1u);
+  }
+};
+unsigned selftest_field_multiply(const EngineCtx& ctx, unsigned threads, unsigned seed) {
+  DevBuf<u32> bad(1, ctx.s);
+  dev_zero(bad.p, sizeof(u32), ctx.s);
+  launch(FieldMulSelfTestBody{seed, bad.p}, threads, ctx.s);
+  u32 host = 0;
+  copy_d2h(&host, bad.p, sizeof(u32), ctx.s);
+  stream_sync(ctx.s);
+  return host;
+}
 void launch_builtin_generators(const EngineCtx& ctx, void* gens, uint64_t first, uint64_t n) {
   launch(BuiltinGeneratorBody{(Ed25519::Gen*)gens, first}, n, ctx.s);
 }

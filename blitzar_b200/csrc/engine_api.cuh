@@ -310,6 +310,9 @@ uint32_t ipa_verify_batch(const EngineCtx& ctx, uint32_t num_proofs, int* result
 // lane-sliced field arithmetic self-test (lanefield.cuh): number of mismatching checks over
 // `warps` warps of pseudo-random / edge-case operands
 unsigned selftest_lane_arithmetic(const EngineCtx& ctx, unsigned warps, unsigned seed);
+// F25519::mul on the device against F25519::mul_ref: number of mismatching products over `threads`
+// operand pairs
+unsigned selftest_field_multiply(const EngineCtx& ctx, unsigned threads, unsigned seed);
 // atomic against binned bucket sort of the same device columns (msm.cuh sort_selftest)
 unsigned selftest_sort(const EngineCtx& ctx, const sxt_sequence_descriptor* d, unsigned num,
                        unsigned window_bits);

@@ -153,27 +153,23 @@ template <int N> B200_HD u32 limbs_sub(u32* r, const u32* a, const u32* b) {
 #endif
 }
 
-// r = a + k (small), returns carry
+// r = a + k (small), returns carry: one add.cc chain on the device (the host runs the same schedule
+// on the emulated carry)
 template <int N> B200_HD u32 limbs_add_small(u32* r, const u32* a, u32 k) {
-  u64 c = k;
+  r[0] = add_cc(a[0], k);
 #pragma unroll
-  for (int i = 0; i < N; ++i) {
-    c += a[i];
-    r[i] = (u32)c;
-    c >>= 32;
-  }
-  return (u32)c;
+  for (int i = 1; i < N; ++i)
+    r[i] = addc_cc(a[i], 0u);
+  return addc(0u, 0u);
 }
 
+// r = a - k (small), returns borrow (0 or 1): one sub.cc chain
 template <int N> B200_HD u32 limbs_sub_small(u32* r, const u32* a, u32 k) {
-  u64 bw = k;
+  r[0] = sub_cc(a[0], k);
 #pragma unroll
-  for (int i = 0; i < N; ++i) {
-    u64 t = (u64)a[i] - bw;
-    r[i] = (u32)t;
-    bw = t >> 63;
-  }
-  return (u32)bw;
+  for (int i = 1; i < N; ++i)
+    r[i] = subc_cc(a[i], 0u);
+  return subc(0u, 0u) & 1u;
 }
 
 template <int N> B200_HD bool limbs_is_zero(const u32* a) {
@@ -252,7 +248,7 @@ struct F25519 {
     fold(r, t);
   }
   // production schedule: 64 wide multiply-adds on even/odd register pairs (mul_wide_eo), one
-  // merge chain, then the 2^256 = 38 fold as a lo pass and a hi pass of mad.cc chains.
+  // merge chain, then the 2^256 = 38 fold as 8 more wide multiply-adds and a merge (fold_cc).
   static B200_HD void mul(E& r, const E& a, const E& b) { mul_school(r, a, b); }
   static B200_HD void mul_school(E& r, const E& a, const E& b) {
     u32 Ev[16], Ov[16], R[16];
@@ -264,25 +260,33 @@ struct F25519 {
       R[k] = addc_cc(Ev[k], Ov[k - 1]);
     fold_cc(r, R);
   }
-  // 16-limb product -> loosely reduced residue, carry-chain form of fold()
+  // 16-limb product -> loosely reduced residue, carry-chain form of fold() with the same result.
+  // The eight products 38 h[k] of the high half h = R[8..16) are 64-bit multiply-adds on register
+  // pairs: even k into (t[k], t[k+1]) on top of R_lo, odd k into a second set of pairs, which one
+  // add chain then merges.
   static B200_HD void fold_cc(E& r, const u32* R) {
-    u32 t[8];
-    t[0] = mad_lo_cc(R[8], 38u, R[0]);
+    const u32* h = R + 8;
+    u32 t[8], u[8];
 #pragma unroll
-    for (int k = 1; k < 8; ++k)
-      t[k] = madc_lo_cc(R[8 + k], 38u, R[k]);
-    u32 c_lo = addc(0u, 0u);
-    t[1] = mad_hi_cc(R[8], 38u, t[1]);
+    for (int k = 0; k < 8; ++k)
+      t[k] = R[k];
+    chain_mad_pairs<4>(t, [h](int k) { return h[2 * k]; }, 38u);
+    u32 top = addc(0u, 0u);
 #pragma unroll
-    for (int k = 1; k < 7; ++k)
-      t[k + 1] = madc_hi_cc(R[8 + k], 38u, t[k + 1]);
-    u32 top = madc_hi(R[15], 38u, c_lo);  // < 2^7
+    for (int k = 0; k < 8; ++k)
+      u[k] = 0;
+    chain_mad_pairs<4>(u, [h](int k) { return h[2 * k + 1]; }, 38u);  // u[k] sits at limb k+1
+    t[1] = add_cc(t[1], u[0]);
+#pragma unroll
+    for (int k = 2; k < 8; ++k)
+      t[k] = addc_cc(t[k], u[k - 1]);
+    top = addc(top, u[7]);  // (R_lo + 38 h) >> 256 <= 38
     r.l[0] = mad_lo_cc(top, 38u, t[0]);
 #pragma unroll
     for (int k = 1; k < 8; ++k)
       r.l[k] = addc_cc(t[k], 0u);
     u32 c2 = addc(0u, 0u);
-    r.l[0] += 38u * c2;  // a wrap leaves a value < 2^12, so this cannot carry
+    r.l[0] += 38u * c2;  // a wrap leaves a value < 2^11, so this cannot carry
   }
 
   static B200_HD void sqr(E& r, const E& a) { mul(r, a, a); }

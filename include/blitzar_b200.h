@@ -285,6 +285,11 @@ uint32_t b200_curve25519_verify_inner_products(
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
+/* Self-test of the curve25519 field multiplier as it runs on the device (carry-chain PTX) against the
+ * plain reference schedule, limb for limb, on `threads` pairs of pseudo-random and edge-case operands
+ * (0, 1, p - 1, p, p + 18, 2^255, 2^256 - 1, ...): returns the number of mismatching products
+ * (0 = pass). */
+unsigned b200_selftest_field_multiply(unsigned threads, unsigned seed);
 /* Self-test of the binned bucket sort: sorts the (term, window) entries of the device-resident
  * columns (window width `window_bits`, 0 = automatic) with the atomic and the binned path and returns
  * the number of buckets whose end offset or entry multiset differs (0 = pass; ~0u when the binned path
