@@ -40,7 +40,7 @@ B200_SYMBOLS = [
     "b200_profile_read", "b200_set_reduce_groups", "b200_stream",
     "b200_synthetic_generators_device", "b200_commit_host_partials",
     "b200_fixed_msm_host_partials", "b200_multiexp_handle_new_device",
-    "b200_selftest_lane_arithmetic", "b200_selftest_field_multiply", "b200_selftest_sort",
+    "b200_selftest_lane_arithmetic", "b200_field_op", "b200_selftest_sort",
     "b200_partition_table_device",
     "b200_multiexp_handle_write_partition_table",
     "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
@@ -337,9 +337,44 @@ def selftest_lane_arithmetic(warps=64, seed=1):
     return int(lib().b200_selftest_lane_arithmetic(C.c_uint(warps), C.c_uint(seed)))
 
 
-def selftest_field_multiply(threads=1 << 16, seed=1):
-    lib().b200_selftest_field_multiply.restype = C.c_uint
-    return int(lib().b200_selftest_field_multiply(C.c_uint(threads), C.c_uint(seed)))
+# b200_field_op: limbs per element of each field, and the operation codes
+FIELD_LIMBS = {0: 8, 1: 12, 2: 8, 3: 8, 4: 8, 5: 10}
+FIELD_OPS = {name: code for code, name in enumerate([
+    "add", "sub", "neg", "dbl", "mul", "mul_ref", "sqr", "mul_lat", "canonical", "is_negative",
+    "invert", "pow22523", "from_radix51", "to_radix51", "sqrt_ratio_m1", "invert_eea", "from_mont",
+    "to_mont", "lexicographically_largest", "carry1", "sub2p", "sub4p", "slice", "gather"])}
+_BINARY_OPS = {"add", "sub", "mul", "mul_ref", "mul_lat", "sqrt_ratio_m1", "sub2p", "sub4p"}
+
+
+def field_op_shape(field, op):
+    """u32 limbs per element of operand a, operand b (0: unary) and the result of field op `op`."""
+    n = FIELD_LIMBS[field]
+    a = {"from_radix51": 10, "slice": 8}.get(op, n)
+    out = {"is_negative": 1, "lexicographically_largest": 1, "to_radix51": 10,
+           "sqrt_ratio_m1": n + 1, "gather": 8}.get(op, n)
+    return a, (n if op in _BINARY_OPS else 0), out
+
+
+def call_field_op(entry, field, op, a, b=None):
+    """Runs a b200_field_op-shaped entry: op (a FIELD_OPS name) on each row of the uint32 arrays a and
+    b; returns the uint32 results [n, limbs]. ValueError when the field does not offer op."""
+    wa, wb, wout = field_op_shape(field, op)
+    a = np.ascontiguousarray(a, dtype=np.uint32).reshape(-1, wa)
+    n = a.shape[0]
+    if wb:
+        b = np.ascontiguousarray(b, dtype=np.uint32).reshape(n, wb)
+    out = np.zeros((n, wout), dtype=np.uint32)
+    entry.restype = C.c_uint
+    rc = entry(C.c_uint(field), C.c_uint(FIELD_OPS[op]), C.c_uint64(n), _ptr(a),
+               _ptr(b if wb else None), _ptr(out))
+    if rc == 0xFFFFFFFF:
+        raise ValueError(f"field {field} does not offer {op}")
+    return out
+
+
+def field_op(field, op, a, b=None):
+    """b200_field_op on the GPU (call_field_op)."""
+    return call_field_op(lib().b200_field_op, field, op, a, b)
 
 
 def selftest_sort(columns_shape, scalar_ptrs, window_bits=0):

@@ -1486,9 +1486,11 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   const Entry entry("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);
 }
-unsigned b200_selftest_field_multiply(unsigned threads, unsigned seed) {
-  const Entry entry("b200_selftest_field_multiply");
-  return selftest_field_multiply(ctx(), threads, seed);
+unsigned b200_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
+                       const uint32_t* b, uint32_t* out) {
+  const Entry entry("b200_field_op");
+  B200_REQUIRE(n == 0 || (a != nullptr && out != nullptr), "null operand or result array");
+  return field_op(ctx(), field, op, n, a, b, out);
 }
 unsigned b200_selftest_sort(const sxt_sequence_descriptor* columns, unsigned num,
                             unsigned window_bits) {

@@ -310,12 +310,31 @@ uint32_t ipa_verify_batch(const EngineCtx& ctx, uint32_t num_proofs, int* result
 // lane-sliced field arithmetic self-test (lanefield.cuh): number of mismatching checks over
 // `warps` warps of pseudo-random / edge-case operands
 unsigned selftest_lane_arithmetic(const EngineCtx& ctx, unsigned warps, unsigned seed);
-// F25519::mul on the device against F25519::mul_ref: number of mismatching products over `threads`
-// operand pairs
-unsigned selftest_field_multiply(const EngineCtx& ctx, unsigned threads, unsigned seed);
 // atomic against binned bucket sort of the same device columns (msm.cuh sort_selftest)
 unsigned selftest_sort(const EngineCtx& ctx, const sxt_sequence_descriptor* d, unsigned num,
                        unsigned window_bits);
+
+// element-wise field arithmetic (field_op.cuh, b200_field_op): `op` on n elements of host arrays,
+// synchronises; ~0u when the field does not offer the operation. Each curve unit runs its own base
+// field (field id = curve id); the ed25519 unit also the scalars mod l (4) and the lane-sliced
+// F25519 (5, device only).
+unsigned field_op_ed25519(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
+                          const uint32_t* a, const uint32_t* b, uint32_t* out);
+unsigned field_op_bls12381(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                           const uint32_t* b, uint32_t* out);
+unsigned field_op_bn254(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                        const uint32_t* b, uint32_t* out);
+unsigned field_op_grumpkin(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                           const uint32_t* b, uint32_t* out);
+inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
+                         const uint32_t* a, const uint32_t* b, uint32_t* out) {
+  switch (field) {
+  case 1: return field_op_bls12381(ctx, op, n, a, b, out);
+  case 2: return field_op_bn254(ctx, op, n, a, b, out);
+  case 3: return field_op_grumpkin(ctx, op, n, a, b, out);
+  default: return field_op_ed25519(ctx, field, op, n, a, b, out);
+  }
+}
 
 // built-in ristretto generators g(first .. first+n) into the device generator layout
 void launch_builtin_generators(const EngineCtx& ctx, void* gens, uint64_t first, uint64_t n);

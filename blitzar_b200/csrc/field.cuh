@@ -605,6 +605,9 @@ template <class P> struct Mont {
   // by two limbs (register renaming). What the move cannot rename — Ov[1], which sits on the new
   // position 0, and the carry bit out of the two zeroed limbs — is added to the new Ev by one
   // N+1-instruction carry chain per frame.
+  // Operands: a < p, b < R (b need not be reduced). The frame holds N + 2 limbs, enough for
+  // t + a (b_i + 2^32 b_i+1) + p (m0 + 2^32 m1) with a < p; an a up to R would need one more, and
+  // its carry out of the top limb would be lost.
   static B200_HD void mul(E& r, const E& a, const E& b) {
     u32 Ev[N + 2], Ov[N + 2];
 #pragma unroll
@@ -797,12 +800,13 @@ template <class P> struct Mont {
     o.l[0] = 1;
     mul(r, a, o);
   }
+  // any a < R (reduces a raw N-limb value): a R mod p
   static B200_HD void to_mont(E& r, const E& a) {
     E r2;
 #pragma unroll
     for (int i = 0; i < N; ++i)
       r2.l[i] = P::r2(i);
-    mul(r, a, r2);
+    mul(r, r2, a);
   }
   // f12p::lexicographically_largest: plain value > (p-1)/2
   static B200_HD bool lexicographically_largest(const E& a) {

@@ -83,7 +83,7 @@ struct IpaReduceBody {
   ScE* v;
   B200_HD void operator()(u64 i) const {
     ScE t;
-    FS::mul(t, v[i], sc_r2());
+    FS::to_mont(t, v[i]);
     FS::from_mont(v[i], t);
   }
 };
@@ -383,7 +383,7 @@ struct IpaLoadBody {
   B200_HD void operator()(u64 i) const {
     const u32 p = seg.of(i);
     ScE t;
-    FS::mul(t, src[i], sc_r2());
+    FS::to_mont(t, src[i]);
     FS::from_mont(dst[dst_off[p] + (i - seg.start[p])], t);
   }
 };

@@ -59,7 +59,8 @@ B200_DEV u32 carry1(const Lane& L, u32 v) {
 }
 B200_DEV u32 add(u32 a, u32 b) { return a + b; }                                  // lazy
 B200_DEV u32 sub2p(const Lane& L, u32 a, u32 b) { return a + L.twop - b; }        // lazy, b reduced
-B200_DEV u32 sub4p(const Lane& L, u32 a, u32 b) { return a + 2u * L.twop - b; }   // lazy, b < 2^27.9
+// lazy; b < 2^27.9 on even limbs, one bit less on odd ones (4p limb-wise: 2^28 - 76, 2^28 - 4 and 2^27 - 4)
+B200_DEV u32 sub4p(const Lane& L, u32 a, u32 b) { return a + 2u * L.twop - b; }
 
 // limb m of a * b mod p. Operand bounds: a, b < 2^27.7 on even limbs, one bit less on odd ones
 // (19 b and 2 a must fit 32 bits, ten products 64); result below 2^26 + 2^22 (2^25 + 2^22).

@@ -285,11 +285,20 @@ uint32_t b200_curve25519_verify_inner_products(
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
-/* Self-test of the curve25519 field multiplier as it runs on the device (carry-chain PTX) against the
- * plain reference schedule, limb for limb, on `threads` pairs of pseudo-random and edge-case operands
- * (0, 1, p - 1, p, p + 18, 2^255, 2^256 - 1, ...): returns the number of mismatching products
- * (0 = pass). */
-unsigned b200_selftest_field_multiply(unsigned threads, unsigned seed);
+/* Test hook: one field operation of the device arithmetic on each of n elements, out[i] = op(a[i],
+ * b[i]). Operands and results are little-endian u32 limbs. Fields: 0 curve25519 Fp (8 limbs, loosely
+ * reduced: any value below 2^256), 1 bls12-381 Fp (12), 2 bn254 Fp (8), 3 grumpkin Fp (8), 4 the
+ * ristretto255 scalars mod l (8), 5 curve25519 Fp lane-sliced over 10 lanes (10 limbs of radix
+ * 2^25.5). Fields 1-4 hold Montgomery residues. Ops: 0 add, 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref,
+ * 6 sqr (fields 0-4); field 0: 7 mul_lat, 8 canonical, 9 is_negative (1 limb out), 10 invert,
+ * 11 pow22523, 12 from_radix51 (10 limbs in: 5 x u64), 13 to_radix51 (10 limbs out),
+ * 14 sqrt_ratio_m1 (a = u, b = v; out: x, then the was-square flag); fields 1-4: 10 invert,
+ * 15 invert_eea, 16 from_mont, 17 to_mont, 18 lexicographically_largest (1 limb out); field 5:
+ * 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p, 22 slice (8 limbs in), 23 gather (8
+ * limbs out). b is read only by binary ops (add, sub, mul, mul_ref, mul_lat, sqrt_ratio_m1, sub2p,
+ * sub4p). Host pointers; synchronises. Returns 0, or ~0u when the field does not offer op. */
+unsigned b200_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
+                       const uint32_t* b, uint32_t* out);
 /* Self-test of the binned bucket sort: sorts the (term, window) entries of the device-resident
  * columns (window width `window_bits`, 0 = automatic) with the atomic and the binned path and returns
  * the number of buckets whose end offset or entry multiset differs (0 = pass; ~0u when the binned path

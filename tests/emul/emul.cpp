@@ -15,6 +15,7 @@
 
 #include "emul_prefix.h"
 #include "../../blitzar_b200/csrc/engine.cuh"
+#include "../../blitzar_b200/csrc/scalar25.h"
 
 using namespace b200;
 
@@ -241,91 +242,38 @@ int emul_verify_inner_product(uint8_t* transcript203, uint64_t n, uint64_t offse
 }
 }
 
-// field-level cross-check: production multiply schedule vs the plain reference schedule
-template <class F> static int check_field(unsigned iters, unsigned seed) {
-  typename F::E a, b, r1, r2;
-  unsigned long long st = seed * 0x9E3779B97F4A7C15ull + 1;
-  auto next = [&st]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return (u32)(st >> 16); };
-  int bad = 0;
-  for (unsigned it = 0; it < iters; ++it) {
-    for (int i = 0; i < F::N; ++i) { a.l[i] = next(); b.l[i] = next(); }
-    if (it % 7 == 0) for (int i = 0; i < F::N; ++i) a.l[i] = 0xffffffffu;
-    if (it % 11 == 0) for (int i = 0; i < F::N; ++i) b.l[i] = 0xffffffffu;
-    if (it % 13 == 0) for (int i = 0; i < F::N; ++i) b.l[i] = 0;
-    // Montgomery operands are residues < p: clear the top bits (p > 2^253 resp. 2^380)
-    a.l[F::N - 1] &= 0x0fffffffu;
-    b.l[F::N - 1] &= 0x0fffffffu;
-    if (it % 17 == 0) { a = F::modulus(); limbs_sub_small<F::N>(a.l, a.l, 1); }
-    if (it % 19 == 0) { b = F::modulus(); limbs_sub_small<F::N>(b.l, b.l, 1 + it % 3); }
-    F::mul(r1, a, b);
-    F::mul_ref(r2, a, b);
-    typename F::E c1 = r1, c2 = r2;
-    bool same = true;
-    for (int i = 0; i < F::N; ++i) same = same && (c1.l[i] == c2.l[i]);
-    if (!same) ++bad;
-  }
-  return bad;
-}
-extern "C" int emul_check_mul(unsigned field_id, unsigned iters, unsigned seed) {
-  switch (field_id) {
-  case 0: {
-    // F25519 results are only congruent mod p; compare canonical forms
-    int bad = 0;
-    F25519::E a, b, r1, r2, c1, c2;
-    unsigned long long st = seed * 0x9E3779B97F4A7C15ull + 1;
-    auto next = [&st]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return (u32)(st >> 16); };
-    for (unsigned it = 0; it < iters; ++it) {
-      for (int i = 0; i < 8; ++i) { a.l[i] = next(); b.l[i] = next(); }
-      if (it % 7 == 0) for (int i = 0; i < 8; ++i) a.l[i] = 0xffffffffu;
-      if (it % 11 == 0) for (int i = 0; i < 8; ++i) b.l[i] = 0xffffffffu;
-      // Karatsuba corner cases: equal / zero halves, halves in either order
-      if (it % 13 == 0) for (int i = 0; i < 4; ++i) a.l[4 + i] = a.l[i];
-      if (it % 17 == 0) for (int i = 0; i < 4; ++i) b.l[i] = b.l[4 + i];
-      if (it % 19 == 0) for (int i = 0; i < 4; ++i) a.l[i] = 0;
-      if (it % 23 == 0) for (int i = 0; i < 4; ++i) b.l[4 + i] = 0;
-      if (it % 29 == 0) for (int i = 0; i < 8; ++i) a.l[i] = 0;
-      F25519::mul(r1, a, b);
-      F25519::mul_ref(r2, a, b);
-      F25519::canonical(c1, r1);
-      F25519::canonical(c2, r2);
-      for (int i = 0; i < 8; ++i) if (c1.l[i] != c2.l[i]) { ++bad; break; }
-      F25519::mul_lat(r1, a, b);
-      F25519::canonical(c1, r1);
-      for (int i = 0; i < 8; ++i) if (c1.l[i] != c2.l[i]) { ++bad; break; }
-    }
-    return bad;
-  }
-  case 1: return check_field<FBls>(iters, seed);
-  case 2: return check_field<FBn>(iters, seed);
-  default: return check_field<FGk>(iters, seed);
-  }
+// same contract as b200_field_op, run on the CPU (~0u for the lane-sliced field, which is device only)
+extern "C" unsigned emul_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
+                                  const uint32_t* b, uint32_t* out) {
+  return field_op(make_ctx(), field, op, n, a, b, out);
 }
 
-// binary-Euclid inversion vs the Fermat power (Montgomery fields), incl. 0, 1, 2, p - 1
-template <class F> static int check_invert(unsigned iters, unsigned seed) {
-  unsigned long long st = seed * 0x9E3779B97F4A7C15ull + 3;
-  auto next = [&st]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return (u32)(st >> 16); };
-  int bad = 0;
-  for (unsigned it = 0; it < iters; ++it) {
-    typename F::E a, r1, r2, one = F::one(), chk;
-    for (int i = 0; i < F::N; ++i) a.l[i] = next();
-    a.l[F::N - 1] &= 0x0fffffffu;
-    if (it == 0) a = F::zero();
-    if (it == 1) a = F::one();
-    if (it == 2) F::add(a, one, one);
-    if (it == 3) { a = F::modulus(); limbs_sub_small<F::N>(a.l, a.l, 1); }
-    if (it == 4) { a = F::zero(); a.l[0] = 1; }  // plain 1 = R^-1 in the Montgomery domain
-    F::invert(r1, a);
-    F::invert_eea(r2, a);
-    if (!F::equal(r1, r2)) ++bad;
-    if (it) { F::mul(chk, r2, a); if (!F::equal(chk, one)) ++bad; }
+// The host scalar arithmetic of scalar25.h (inner-product challenges and verifier exponents) on n
+// elements of 8 little-endian u32 limbs: 0 sc_reduce(a), 1 sc_mul(a, b), 2 sc_mul_mont(sc_to_mont(a),
+// b), 3 sc_add, 4 sc_sub, 5 sc_neg(a), 6 sc_inv(a), 7 sc_inner_product of all n pairs (one result).
+// Returns 0, or ~0u for an unknown op.
+extern "C" unsigned emul_scalar_op(unsigned op, uint64_t n, const uint32_t* a, const uint32_t* b,
+                                   uint32_t* out) {
+  if (op == 7) {
+    sc_store((uint8_t*)out, sc_inner_product((const uint8_t*)a, (const uint8_t*)b, n));
+    return 0;
   }
-  return bad;
-}
-extern "C" int emul_check_invert(unsigned field_id, unsigned iters, unsigned seed) {
-  switch (field_id) {
-  case 1: return check_invert<FBls>(iters, seed);
-  case 2: return check_invert<FBn>(iters, seed);
-  default: return check_invert<FGk>(iters, seed);
+  if (op > 7)
+    return ~0u;
+  for (uint64_t i = 0; i < n; ++i) {
+    const Sc x = sc_load((const uint8_t*)(a + 8 * i));
+    const Sc y = b ? sc_load((const uint8_t*)(b + 8 * i)) : sc_zero();
+    Sc r;
+    switch (op) {
+    case 0: r = sc_reduce(x); break;
+    case 1: r = sc_mul(x, y); break;
+    case 2: r = sc_mul_mont(sc_to_mont(x), y); break;
+    case 3: r = sc_add(x, y); break;
+    case 4: r = sc_sub(x, y); break;
+    case 5: r = sc_neg(x); break;
+    default: r = sc_inv(x); break;
+    }
+    sc_store((uint8_t*)(out + 8 * i), r);
   }
+  return 0;
 }

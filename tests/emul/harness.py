@@ -12,7 +12,8 @@ import ctypes as C
 import numpy as np
 
 from blitzar_b200 import build as _build
-from blitzar_b200.api import COMPACT_BYTES, CURVE_SIZES, make_descriptors, partition_table_bytes
+from blitzar_b200.api import (COMPACT_BYTES, CURVE_SIZES, call_field_op, make_descriptors,
+                               partition_table_bytes)
 
 # partition_policy: outputs of a fixed MSM over a handle with a partition table are answered from
 # the table as the cost model decides, all of them, or none
@@ -188,12 +189,27 @@ def synth_generators(curve_id, n, first=0, projective=False):
     return out
 
 
-def check_mul(field_id, iters=2000, seed=1):
-    return int(lib().emul_check_mul(C.c_uint(field_id), C.c_uint(iters), C.c_uint(seed)))
+def field_op(field, op, a, b=None):
+    """emul_field_op: b200_field_op's contract (blitzar_b200.api.call_field_op) on the CPU."""
+    return call_field_op(lib().emul_field_op, field, op, a, b)
 
 
-def check_invert(field_id, iters=300, seed=1):
-    return int(lib().emul_check_invert(C.c_uint(field_id), C.c_uint(iters), C.c_uint(seed)))
+SCALAR_OPS = {name: code for code, name in enumerate(
+    ["reduce", "mul", "mul_mont", "add", "sub", "neg", "inv", "inner_product"])}
+
+
+def scalar_op(op, a, b=None):
+    """emul_scalar_op: the host scalar arithmetic mod l (scalar25.h) on rows of 8 u32 limbs;
+    inner_product returns the one sum over all rows."""
+    a = np.ascontiguousarray(a, dtype=np.uint32).reshape(-1, 8)
+    if b is not None:
+        b = np.ascontiguousarray(b, dtype=np.uint32).reshape(a.shape)
+    out = np.zeros((1 if op == "inner_product" else a.shape[0], 8), dtype=np.uint32)
+    lib().emul_scalar_op.restype = C.c_uint
+    rc = lib().emul_scalar_op(C.c_uint(SCALAR_OPS[op]), C.c_uint64(a.shape[0]), _ptr(a), _ptr(b),
+                              _ptr(out))
+    assert rc == 0, op
+    return out
 
 
 def prove_inner_product(transcript, a, b, generators_offset=0):

@@ -8,17 +8,6 @@ import pytest
 from tests import common
 
 
-def test_production_multiply_schedules_match_reference_schedules(emul):
-    # F25519, bls12-381, bn254, grumpkin: carry-chain even/odd schedule vs plain 64-bit schedule
-    for field_id in range(4):
-        assert emul.check_mul(field_id, 4000, seed=field_id + 1) == 0
-
-
-def test_binary_euclid_inversion_matches_fermat(emul):
-    for field_id in (1, 2, 3):
-        assert emul.check_invert(field_id, 300, field_id) == 0
-
-
 def test_golden_commitments(emul):
     assert emul.commit(0, common.golden_columns()).tolist() == common.GOLDEN_COMMITMENTS
 
