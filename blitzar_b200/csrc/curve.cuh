@@ -1,4 +1,4 @@
-// Group law for the four curves of the MSM hot path, as device functions over field.cuh.
+// Group law for the curves of the MSM hot path, as device functions over field.cuh.
 //
 // Replaces (re-derived): sxt/curve21 (+ sxt/ristretto compress / elligator), sxt/curve_g1,
 // sxt/curve_bng1, sxt/curve_gk — the `add / double / neg / identity` concept of
@@ -16,7 +16,13 @@
 
 namespace b200 {
 
-enum CurveId : unsigned { kRistretto255 = 0, kBls12381 = 1, kBn254 = 2, kGrumpkin = 3 };
+enum CurveId : unsigned {
+  kRistretto255 = 0,
+  kBls12381 = 1,
+  kBn254 = 2,
+  kGrumpkin = 3,
+  kBls12381G2 = 4,  // no counterpart in the reference, which defines ids 0-3
+};
 
 // ---- execution policies for the independent field multiplications inside a point operation -------
 // SeqExec : one thread computes every product (throughput-bound kernels).
@@ -804,7 +810,44 @@ struct BlsCurveParams {
   }
 };
 
+// bls12-381 G2: y^2 = x^3 + 4 (1 + u) over Fp2Bls
+struct Bls2CurveParams {
+  static constexpr unsigned kCurveId = kBls12381G2;
+  static constexpr int kAbiAffineStride = 200;  // {X[12], Y[12], u8 infinity}, padded to 8 bytes
+  static constexpr int kAbiCommitBytes = 96;
+  // 3b = 12 (1 + u)
+  template <class F> static B200_HD void mul_by_3b(typename F::E& r, const typename F::E& a) {
+    typename F::E t;
+    F::mul_by_1pu(t, a);
+    BlsCurveParams::mul_by_3b<F>(r, t);
+  }
+  // zcash-style 96-byte compressed encoding (what blst, arkworks and zkcrypto read): x.c1 then x.c0,
+  // 48 bytes each, big-endian; flags in the top bits of byte 0 as for G1
+  template <class W> static B200_HD void store_commit(void* dst, const typename W::Point& p) {
+    typename W::fe x, y, xp;
+    bool inf = W::to_affine(x, y, p);
+    if (inf)
+      x = W::F::zero();
+    W::F::from_mont(xp, x);
+    unsigned char* d = (unsigned char*)dst;
+#pragma unroll
+    for (int i = 0; i < 24; ++i) {  // c1 in limbs 12..23 above c0: the 768-bit value c0 + 2^384 c1
+      u32 w = xp.l[23 - i];
+      d[4 * i] = (unsigned char)(w >> 24);
+      d[4 * i + 1] = (unsigned char)(w >> 16);
+      d[4 * i + 2] = (unsigned char)(w >> 8);
+      d[4 * i + 3] = (unsigned char)w;
+    }
+    d[0] |= 0x80;
+    if (inf)
+      d[0] |= 0x40;
+    else if (W::F::lexicographically_largest(y))
+      d[0] |= 0x20;
+  }
+};
+
 typedef Weierstrass<FBls, BlsCurveParams> Bls12381G1;
+typedef Weierstrass<Fp2Bls, Bls2CurveParams> Bls12381G2;
 typedef Weierstrass<FBn, BnCurveParams> Bn254G1;
 typedef Weierstrass<FGk, GkCurveParams> GrumpkinG;
 

@@ -1,4 +1,5 @@
-// Prime-field arithmetic on 32-bit limbs for the four curves of the MSM hot path.
+// Prime-field arithmetic on 32-bit limbs for the curves of the MSM hot path, and the quadratic
+// extension Fp2 of the bls12-381 base field that G2 is defined over.
 //
 // Replaces (re-derived, not translated): sxt/field51/operation/{mul,sq,add,sub}.cc (radix-2^51
 // curve25519 field), sxt/field12 (bls12-381), sxt/field25 (bn254), sxt/fieldgk (grumpkin) and
@@ -881,5 +882,184 @@ typedef Mont<Sc25Params> FSc25;
 typedef Mont<BnParams> FBn;
 typedef Mont<GkParams> FGk;
 typedef Mont<BlsParams> FBls;
+
+// ------------------------------------------------------------------------------------------------
+// Fp2Bls: Fp2 = Fp[u] / (u^2 + 1) over the bls12-381 base field, the field of G2. An element
+// c0 + c1 u is one Fe<24>: c0 in l[0..11], c1 in l[12..23], each a Montgomery residue of FBls
+// (R = 2^384). That is the layout of the reference-style {X, Y} structs as well (c0 limbs first), and
+// it lets Weierstrass<> index, load and store it like any N-limb field.
+// ------------------------------------------------------------------------------------------------
+struct Bls2Params {  // the G2 generator (IETF BLS / zcash), Montgomery c0 then c1
+  static B200_HD u32 gx(int i) { return BLS2_GX(i); }
+  static B200_HD u32 gy(int i) { return BLS2_GY(i); }
+};
+struct Fp2Bls {
+  typedef Bls2Params Params;
+  typedef FBls B;
+  typedef B::E Be;
+  static constexpr int H = B::N;  // limbs of one component
+  static constexpr int N = 2 * H;
+  typedef Fe<N> E;
+
+  static B200_HD Be part(const E& a, int k) {
+    Be r;
+#pragma unroll
+    for (int i = 0; i < H; ++i)
+      r.l[i] = a.l[k * H + i];
+    return r;
+  }
+  static B200_HD void join(E& r, const Be& c0, const Be& c1) {
+#pragma unroll
+    for (int i = 0; i < H; ++i) {
+      r.l[i] = c0.l[i];
+      r.l[H + i] = c1.l[i];
+    }
+  }
+
+  static B200_HD E zero() {
+    E r;
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      r.l[i] = 0;
+    return r;
+  }
+  static B200_HD E one() {
+    E r;
+    join(r, B::one(), B::zero());
+    return r;
+  }
+  static B200_HD void add(E& r, const E& a, const E& b) {
+    Be c0, c1;
+    B::add(c0, part(a, 0), part(b, 0));
+    B::add(c1, part(a, 1), part(b, 1));
+    join(r, c0, c1);
+  }
+  static B200_HD void sub(E& r, const E& a, const E& b) {
+    Be c0, c1;
+    B::sub(c0, part(a, 0), part(b, 0));
+    B::sub(c1, part(a, 1), part(b, 1));
+    join(r, c0, c1);
+  }
+  static B200_HD void neg(E& r, const E& a) {
+    Be c0, c1;
+    B::neg(c0, part(a, 0));
+    B::neg(c1, part(a, 1));
+    join(r, c0, c1);
+  }
+  static B200_HD void dbl(E& r, const E& a) { add(r, a, a); }
+  // r = a (1 + u) = (a0 - a1) + (a0 + a1) u
+  static B200_HD void mul_by_1pu(E& r, const E& a) {
+    Be c0, c1;
+    const Be a0 = part(a, 0), a1 = part(a, 1);
+    B::sub(c0, a0, a1);
+    B::add(c1, a0, a1);
+    join(r, c0, c1);
+  }
+  static B200_HD bool is_zero(const E& a) { return limbs_is_zero<N>(a.l); }
+  static B200_HD bool equal(const E& a, const E& b) {
+    u32 x = 0;
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      x |= a.l[i] ^ b.l[i];
+    return x == 0;
+  }
+  static B200_HD void select(E& r, const E& a, const E& b, bool pick_b) {
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      r.l[i] = pick_b ? b.l[i] : a.l[i];
+  }
+
+  // The product and the square are called, not inlined: a G2 point operation holds a dozen of them,
+  // and inlining three 12-limb Montgomery products into each made the G2 unit take half an hour to
+  // compile (cicc), where called bodies compile once.
+  // Karatsuba: v0 = a0 b0, v1 = a1 b1, c0 = v0 - v1, c1 = (a0 + a1)(b0 + b1) - v0 - v1; three base
+  // multiplications, every operand reduced (< p)
+  static __host__ __device__ __attribute__((noinline)) void mul(E& r, const E& a, const E& b) {
+    Be v0, v1, s, t, c0, c1;
+    const Be a0 = part(a, 0), a1 = part(a, 1), b0 = part(b, 0), b1 = part(b, 1);
+    B::mul(v0, a0, b0);
+    B::mul(v1, a1, b1);
+    B::add(s, a0, a1);
+    B::add(t, b0, b1);
+    B::mul(c1, s, t);
+    B::sub(c1, c1, v0);
+    B::sub(c1, c1, v1);
+    B::sub(c0, v0, v1);
+    join(r, c0, c1);
+  }
+  static B200_HD void mul_lat(E& r, const E& a, const E& b) { mul(r, a, b); }
+  // reference schedule: the schoolbook form (four products) over the base field's reference product
+  static B200_HD void mul_ref(E& r, const E& a, const E& b) {
+    Be p00, p11, p01, p10, c0, c1;
+    const Be a0 = part(a, 0), a1 = part(a, 1), b0 = part(b, 0), b1 = part(b, 1);
+    B::mul_ref(p00, a0, b0);
+    B::mul_ref(p11, a1, b1);
+    B::mul_ref(p01, a0, b1);
+    B::mul_ref(p10, a1, b0);
+    B::sub(c0, p00, p11);
+    B::add(c1, p01, p10);
+    join(r, c0, c1);
+  }
+  // (a0 + a1)(a0 - a1) + 2 a0 a1 u: two base multiplications
+  static __host__ __device__ __attribute__((noinline)) void sqr(E& r, const E& a) {
+    Be s, d, c0, c1;
+    const Be a0 = part(a, 0), a1 = part(a, 1);
+    B::add(s, a0, a1);
+    B::sub(d, a0, a1);
+    B::mul(c0, s, d);
+    B::mul(c1, a0, a1);
+    B::dbl(c1, c1);
+    join(r, c0, c1);
+  }
+
+  // 1 / a = (a0 - a1 u) / (a0^2 + a1^2) (0 -> 0): one base inversion of the norm
+  template <bool kEea> static B200_HD void invert_by_norm(E& r, const E& a) {
+    Be n, t, c0, c1;
+    const Be a0 = part(a, 0), a1 = part(a, 1);
+    B::sqr(n, a0);
+    B::sqr(t, a1);
+    B::add(n, n, t);
+    if (kEea)
+      B::invert_eea(t, n);
+    else
+      B::invert(t, n);
+    B::mul(c0, a0, t);
+    B::mul(c1, a1, t);
+    B::neg(c1, c1);
+    join(r, c0, c1);
+  }
+  static B200_HD void invert(E& r, const E& a) { invert_by_norm<false>(r, a); }
+  static B200_HD void invert_eea(E& r, const E& a) { invert_by_norm<true>(r, a); }
+
+  static B200_HD void from_mont(E& r, const E& a) {
+    Be c0, c1;
+    B::from_mont(c0, part(a, 0));
+    B::from_mont(c1, part(a, 1));
+    join(r, c0, c1);
+  }
+  static B200_HD void to_mont(E& r, const E& a) {
+    Be c0, c1;
+    B::to_mont(c0, part(a, 0));
+    B::to_mont(c1, part(a, 1));
+    join(r, c0, c1);
+  }
+  // the zcash rule: c1 decides, unless it is zero; then c0 does
+  static B200_HD bool lexicographically_largest(const E& a) {
+    const Be a0 = part(a, 0), a1 = part(a, 1);
+    return B::is_zero(a1) ? B::lexicographically_largest(a0) : B::lexicographically_largest(a1);
+  }
+  static B200_HD void load(E& r, const void* src) {
+    const u32* s = (const u32*)src;
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      r.l[i] = s[i];
+  }
+  static B200_HD void store(void* dst, const E& a) {
+    u32* d = (u32*)dst;
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+      d[i] = a.l[i];
+  }
+};
 
 }  // namespace b200

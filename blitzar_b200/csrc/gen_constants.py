@@ -70,6 +70,11 @@ def sqrt_mod(n, p):
 # grumpkin (1, sqrt(-16)) with the smaller root
 BLS_GX = 3685416753713387016781088315183077757961620795782546409894578378688607592378376318836054947676345821548104185464507
 BLS_GY = 1339506544944476473020471379941921221584933875938349620426543736416511423956333506472724655353366534992391756441569
+# the G2 generator of bls12-381 (IETF BLS signatures / zcash), coordinates c0 + c1 u in Fp2 = Fp[u]/(u^2 + 1)
+BLS2_GX = (0x024aa2b2f08f0a91260805272dc51051c6e47ad4fa403b02b4510b647ae3d1770bac0326a805bbefd48056c8c121bdb8,
+           0x13e02b6052719f607dacd3a088274f65596bd0d09920b61ab5da61bbdc7f5049334cf11213945d57e5ac7d055d042b7e)
+BLS2_GY = (0x0ce5d527727d6e118cc9cdc6da2e351aadfd9baa8cbdd3a76d429a695160d12c923ac9cc3baca289e193548608b82801,
+           0x0606c4a02ea734cc32acd2b02bc28b99cb3e287e85a763af267492ab572e99ab3f370d275cec1da1aaa9075ff05f79be)
 
 
 def mont_block(prefix, p, n, b, gx, gy):
@@ -88,6 +93,21 @@ def mont_block(prefix, p, n, b, gx, gy):
     out.append(table(f"{prefix}_GX", gx * R % p, n))        # subgroup generator, Montgomery form
     out.append(table(f"{prefix}_GY", gy * R % p, n))
     return "\n".join(out)
+
+
+def fp2_block(prefix, p, n, b, gx, gy):
+    """The generator of a curve y^2 = x^3 + b over Fp2 = Fp[u]/(u^2 + 1), b and the coordinates as
+    (c0, c1): 2n limbs per coordinate, the Montgomery c0 (R = 2^(32 n)) then c1."""
+    def mul(x, y):
+        return ((x[0] * y[0] - x[1] * y[1]) % p, (x[0] * y[1] + x[1] * y[0]) % p)
+    x3 = mul(mul(gx, gx), gx)
+    assert mul(gy, gy) == ((x3[0] + b[0]) % p, (x3[1] + b[1]) % p)
+    R = 1 << (32 * n)
+
+    def mont(v):
+        return v[0] * R % p + (v[1] * R % p << (32 * n))
+    return "\n".join([f"// ---- {prefix}: generator of y^2 = x^3 + ({b[0]} + {b[1]} u) over Fp2, p = 0x{p:x}",
+                      table(f"{prefix}_GX", mont(gx), 2 * n), table(f"{prefix}_GY", mont(gy), 2 * n)])
 
 
 L25519 = 2**252 + 27742317777372353535851937790883648493  # order of the ristretto255 group
@@ -129,6 +149,7 @@ def main():
     parts.append(mont_block("BN", BN254_Q, 8, 3, 1, 2))
     parts.append(mont_block("GK", BN254_R, 8, -17, 1, sqrt_mod(-16 % BN254_R, BN254_R)))
     parts.append(mont_block("BLS", BLS_Q, 12, 4, BLS_GX, BLS_GY))
+    parts.append(fp2_block("BLS2", BLS_Q, 12, (4, 4), BLS2_GX, BLS2_GY))
     parts.append(scalar_block("SC25", L25519, 8))
     parts.append("}  // namespace b200")
     here = os.path.dirname(os.path.abspath(__file__))

@@ -153,6 +153,20 @@ void sxt_prove_sumcheck(void* polynomials, void* evaluation_point, unsigned fiel
 
 /* ---- Part 2: device-resident extension ---- */
 
+/* bls12-381 G2 (y^2 = x^3 + 4(1 + u) over Fp2 = Fp[u]/(u^2 + 1)), accepted as curve_id by every call
+ * that takes a curve id or a handle except those defined for ristretto255 only (built-in generators,
+ * inner-product arguments). The reference defines curve ids 0-3 only; this one has no counterpart
+ * there. Coordinates are Fp2 elements c0 + c1 u as 12 Montgomery limbs (R = 2^384) of c0, then 12 of
+ * c1. Commitment generators (and the affine synthetic generators) are b200_bls12_381_g2, 200 bytes
+ * each; handle generators and fixed-MSM results are b200_bls12_381_g2_p2 (projective, identity Z = 0);
+ * commitments are the 96-byte zcash compressed encoding (x.c1 then x.c0, big-endian; flags 0x80
+ * compressed, 0x40 infinity, 0x20 lexicographically largest y), as blst, arkworks and zkcrypto read
+ * it. b200_field_op's field 6 is this Fp2. */
+#define B200_CURVE_BLS12_381_G2 4
+struct b200_bls12_381_g2 { uint64_t X[12]; uint64_t Y[12]; uint8_t infinity; };
+struct b200_bls12_381_g2_p2 { uint64_t X[12]; uint64_t Y[12]; uint64_t Z[12]; };
+struct b200_bls12_381_g2_compressed { uint8_t g2_bytes[96]; };
+
 /* Bind the calling thread / library to a CUDA device before sxt_init (default: current device). */
 void b200_set_device(int device);
 /* Number of kernels this library has launched so far in this process. */
@@ -289,12 +303,12 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
  * b[i]). Operands and results are little-endian u32 limbs. Fields: 0 curve25519 Fp (8 limbs, loosely
  * reduced: any value below 2^256), 1 bls12-381 Fp (12), 2 bn254 Fp (8), 3 grumpkin Fp (8), 4 the
  * ristretto255 scalars mod l (8), 5 curve25519 Fp lane-sliced over 10 lanes (10 limbs of radix
- * 2^25.5). Fields 1-4 hold Montgomery residues. Ops: 0 add, 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref,
- * 6 sqr (fields 0-4); field 0: 7 mul_lat, 8 canonical, 9 is_negative (1 limb out), 10 invert,
- * 11 pow22523, 12 from_radix51 (10 limbs in: 5 x u64), 13 to_radix51 (10 limbs out),
- * 14 sqrt_ratio_m1 (a = u, b = v; out: x, then the was-square flag); fields 1-4: 10 invert,
- * 15 invert_eea, 16 from_mont, 17 to_mont, 18 lexicographically_largest (1 limb out); field 5:
- * 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p, 22 slice (8 limbs in), 23 gather (8
+ * 2^25.5), 6 bls12-381 Fp2 (24: c0 then c1). Fields 1-4 and 6 hold Montgomery residues. Ops: 0 add,
+ * 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref, 6 sqr (fields 0-4, 6); field 0: 7 mul_lat, 8 canonical,
+ * 9 is_negative (1 limb out), 10 invert, 11 pow22523, 12 from_radix51 (10 limbs in: 5 x u64),
+ * 13 to_radix51 (10 limbs out), 14 sqrt_ratio_m1 (a = u, b = v; out: x, then the was-square flag);
+ * fields 1-4 and 6: 10 invert, 15 invert_eea, 16 from_mont, 17 to_mont, 18 lexicographically_largest
+ * (1 limb out; field 6: the zcash rule, c1 decides unless it is 0); field 5: 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p, 22 slice (8 limbs in), 23 gather (8
  * limbs out). b is read only by binary ops (add, sub, mul, mul_ref, mul_lat, sqrt_ratio_m1, sub2p,
  * sub4p). Host pointers; synchronises. Returns 0, or ~0u when the field does not offer op. */
 unsigned b200_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
