@@ -14,12 +14,14 @@ LIB_PATH = os.path.join(_HERE, "lib", "libblitzar_b200.so")
 SXT_CPU_BACKEND, SXT_GPU_BACKEND = 1, 2
 SXT_CURVE_RISTRETTO255, SXT_CURVE_BLS_381, SXT_CURVE_BN_254, SXT_CURVE_GRUMPKIN = 0, 1, 2, 3
 B200_CURVE_BLS12_381_G2 = 4  # this library's own id: the reference has no G2
+B200_CURVE_BN254_G2 = 5  # likewise
+G2_CURVES = (B200_CURVE_BLS12_381_G2, B200_CURVE_BN254_G2)
 # per curve: (projective ABI bytes, commitment-generator stride, commitment output bytes)
 CURVE_SIZES = {0: (160, 160, 32), 1: (144, 104, 48), 2: (96, 72, 72), 3: (96, 72, 72),
-               4: (288, 200, 96)}
+               4: (288, 200, 96), 5: (192, 136, 136)}
 # bytes of one entry of the reference's partition tables (c21t / cg1t / cn1t / cgkt::compact_element),
 # and of the same {X, Y} layout over G2's Fp2 coordinates
-COMPACT_BYTES = {0: 120, 1: 96, 2: 64, 3: 64, 4: 192}
+COMPACT_BYTES = {0: 120, 1: 96, 2: 64, 3: 64, 4: 192, 5: 128}
 
 SXT_SYMBOLS = [
     "sxt_init", "sxt_curve25519_compute_pedersen_commitments",
@@ -128,12 +130,12 @@ def _ptr(a):
 
 def compute_pedersen_commitments(curve_id, columns, generators=None, offset_generators=0):
     """The five sxt_*_compute_pedersen_commitments* entry points behind one Python call, and for
-    bls12-381 G2 (curve 4, no sxt_* entry point) b200_compute_pedersen_commitments_with_offsets.
+    the G2 curves (4 and 5, no sxt_* entry point) b200_compute_pedersen_commitments_with_offsets.
 
     generators: uint8 array [n, stride] in the ABI layout of the curve (None = built-in ristretto
     generators at offset_generators). Returns uint8 [num_columns, commitment bytes].
     """
-    if curve_id == B200_CURVE_BLS12_381_G2:
+    if curve_id in G2_CURVES:
         return compute_pedersen_commitments_with_offsets(curve_id, columns, None, generators)
     L = lib()
     desc, keep = make_descriptors(columns)
@@ -344,7 +346,7 @@ def selftest_lane_arithmetic(warps=64, seed=1):
 
 
 # b200_field_op: limbs per element of each field, and the operation codes
-FIELD_LIMBS = {0: 8, 1: 12, 2: 8, 3: 8, 4: 8, 5: 10, 6: 24}
+FIELD_LIMBS = {0: 8, 1: 12, 2: 8, 3: 8, 4: 8, 5: 10, 6: 24, 7: 16}
 FIELD_OPS = {name: code for code, name in enumerate([
     "add", "sub", "neg", "dbl", "mul", "mul_ref", "sqr", "mul_lat", "canonical", "is_negative",
     "invert", "pow22523", "from_radix51", "to_radix51", "sqrt_ratio_m1", "invert_eea", "from_mont",

@@ -14,7 +14,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", "-O3"] + ARCH + ["-lineinfo",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC"]
 UNITS = ["api.cu", "curve_ed25519.cu", "curve_bls12381.cu", "curve_bn254.cu", "curve_grumpkin.cu",
-         "curve_bls12381_g2.cu"]
+         "curve_bls12381_g2.cu", "curve_bn254_g2.cu"]
 
 
 def _newer(target, sources):

@@ -271,7 +271,7 @@ struct CurveVTable {
                          uint64_t first_group, uint64_t groups, void* out_gens);
 };
 extern const CurveVTable kVTableEd25519, kVTableBls12381, kVTableBn254, kVTableGrumpkin,
-    kVTableBls12381G2;
+    kVTableBls12381G2, kVTableBn254G2;
 
 inline const CurveVTable& curve_vtable(unsigned curve_id) {
   switch (curve_id) {
@@ -285,6 +285,8 @@ inline const CurveVTable& curve_vtable(unsigned curve_id) {
     return kVTableGrumpkin;
   case B200_CURVE_BLS12_381_G2:
     return kVTableBls12381G2;
+  case B200_CURVE_BN254_G2:
+    return kVTableBn254G2;
   default:
     die("unsupported curve id", __FILE__, __LINE__);
   }
@@ -319,8 +321,8 @@ unsigned selftest_sort(const EngineCtx& ctx, const sxt_sequence_descriptor* d, u
 
 // element-wise field arithmetic (field_op.cuh, b200_field_op): `op` on n elements of host arrays,
 // synchronises; ~0u when the field does not offer the operation. Each curve unit runs its own base
-// field (field id = curve id, except G2's Fp2: 6); the ed25519 unit also the scalars mod l (4) and the
-// lane-sliced F25519 (5, device only).
+// field (field id = curve id, except the G2 Fp2s: bls12-381 6, bn254 7); the ed25519 unit also the
+// scalars mod l (4) and the lane-sliced F25519 (5, device only).
 unsigned field_op_ed25519(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
                           const uint32_t* a, const uint32_t* b, uint32_t* out);
 unsigned field_op_bls12381(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
@@ -331,6 +333,8 @@ unsigned field_op_grumpkin(const EngineCtx& ctx, unsigned op, uint64_t n, const 
                            const uint32_t* b, uint32_t* out);
 unsigned field_op_bls12381_g2(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
                               const uint32_t* b, uint32_t* out);
+unsigned field_op_bn254_g2(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                           const uint32_t* b, uint32_t* out);
 inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
                          const uint32_t* a, const uint32_t* b, uint32_t* out) {
   switch (field) {
@@ -338,6 +342,7 @@ inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint
   case 2: return field_op_bn254(ctx, op, n, a, b, out);
   case 3: return field_op_grumpkin(ctx, op, n, a, b, out);
   case 6: return field_op_bls12381_g2(ctx, op, n, a, b, out);
+  case 7: return field_op_bn254_g2(ctx, op, n, a, b, out);
   default: return field_op_ed25519(ctx, field, op, n, a, b, out);
   }
 }

@@ -1,5 +1,5 @@
 // Prime-field arithmetic on 32-bit limbs for the curves of the MSM hot path, and the quadratic
-// extension Fp2 of the bls12-381 base field that G2 is defined over.
+// extensions Fp2 of the bls12-381 and bn254 base fields that their G2 groups are defined over.
 //
 // Replaces (re-derived, not translated): sxt/field51/operation/{mul,sq,add,sub}.cc (radix-2^51
 // curve25519 field), sxt/field12 (bls12-381), sxt/field25 (bn254), sxt/fieldgk (grumpkin) and
@@ -884,19 +884,23 @@ typedef Mont<GkParams> FGk;
 typedef Mont<BlsParams> FBls;
 
 // ------------------------------------------------------------------------------------------------
-// Fp2Bls: Fp2 = Fp[u] / (u^2 + 1) over the bls12-381 base field, the field of G2. An element
-// c0 + c1 u is one Fe<24>: c0 in l[0..11], c1 in l[12..23], each a Montgomery residue of FBls
-// (R = 2^384). That is the layout of the reference-style {X, Y} structs as well (c0 limbs first), and
-// it lets Weierstrass<> index, load and store it like any N-limb field.
+// Fp2<B, P>: Fp2 = Fp[u] / (u^2 + 1) over a Montgomery base field B, the field of a G2. Both base
+// primes here are 3 mod 4, so -1 is a non-residue and u^2 = -1 gives the extension. An element
+// c0 + c1 u is one Fe<2 B::N>: c0 in the low B::N limbs, c1 in the high ones, each a Montgomery
+// residue of B. That is the layout of the reference-style {X, Y} structs as well (c0 limbs first), and
+// it lets Weierstrass<> index, load and store it like any N-limb field. P supplies the G2 generator.
 // ------------------------------------------------------------------------------------------------
-struct Bls2Params {  // the G2 generator (IETF BLS / zcash), Montgomery c0 then c1
+struct Bls2Params {  // the bls12-381 G2 generator (IETF BLS / zcash), Montgomery c0 then c1
   static B200_HD u32 gx(int i) { return BLS2_GX(i); }
   static B200_HD u32 gy(int i) { return BLS2_GY(i); }
 };
-struct Fp2Bls {
-  typedef Bls2Params Params;
-  typedef FBls B;
-  typedef B::E Be;
+struct Bn2Params {  // the bn254 G2 generator (EIP-197), Montgomery c0 then c1
+  static B200_HD u32 gx(int i) { return BN2_GX(i); }
+  static B200_HD u32 gy(int i) { return BN2_GY(i); }
+};
+template <class B, class P> struct Fp2 {
+  typedef P Params;
+  typedef typename B::E Be;
   static constexpr int H = B::N;  // limbs of one component
   static constexpr int N = 2 * H;
   typedef Fe<N> E;
@@ -947,7 +951,7 @@ struct Fp2Bls {
     join(r, c0, c1);
   }
   static B200_HD void dbl(E& r, const E& a) { add(r, a, a); }
-  // r = a (1 + u) = (a0 - a1) + (a0 + a1) u
+  // r = a (1 + u) = (a0 - a1) + (a0 + a1) u (the bls12-381 twist's 3b' = 12 (1 + u))
   static B200_HD void mul_by_1pu(E& r, const E& a) {
     Be c0, c1;
     const Be a0 = part(a, 0), a1 = part(a, 1);
@@ -970,8 +974,8 @@ struct Fp2Bls {
   }
 
   // The product and the square are called, not inlined: a G2 point operation holds a dozen of them,
-  // and inlining three 12-limb Montgomery products into each made the G2 unit take half an hour to
-  // compile (cicc), where called bodies compile once.
+  // and inlining three 12-limb Montgomery products into each made the bls12-381 G2 unit take half an
+  // hour to compile (cicc), where called bodies compile once.
   // Karatsuba: v0 = a0 b0, v1 = a1 b1, c0 = v0 - v1, c1 = (a0 + a1)(b0 + b1) - v0 - v1; three base
   // multiplications, every operand reduced (< p)
   static __host__ __device__ __attribute__((noinline)) void mul(E& r, const E& a, const E& b) {
@@ -1061,5 +1065,7 @@ struct Fp2Bls {
       d[i] = a.l[i];
   }
 };
+typedef Fp2<FBls, Bls2Params> Fp2Bls;  // bls12-381 G2 (R = 2^384 per component)
+typedef Fp2<FBn, Bn2Params> Fp2Bn;     // bn254 G2 (R = 2^256 per component)
 
 }  // namespace b200

@@ -75,6 +75,13 @@ BLS2_GX = (0x024aa2b2f08f0a91260805272dc51051c6e47ad4fa403b02b4510b647ae3d1770ba
            0x13e02b6052719f607dacd3a088274f65596bd0d09920b61ab5da61bbdc7f5049334cf11213945d57e5ac7d055d042b7e)
 BLS2_GY = (0x0ce5d527727d6e118cc9cdc6da2e351aadfd9baa8cbdd3a76d429a695160d12c923ac9cc3baca289e193548608b82801,
            0x0606c4a02ea734cc32acd2b02bc28b99cb3e287e85a763af267492ab572e99ab3f370d275cec1da1aaa9075ff05f79be)
+# the G2 generator of bn254 (EIP-197, which lists the u coefficient first), as c0 + c1 u; its twist is
+# y^2 = x^3 + 3 / (9 + u)
+BN2_GX = (10857046999023057135944570762232829481370756359578518086990519993285655852781,
+          11559732032986387107991004021392285783925812861821192530917403151452391805634)
+BN2_GY = (8495653923123431417604973247489272438418190587263600148770280649306958101930,
+          4082367875863433681332203403145435568316851327593401208105741076214120093531)
+BN2_B = (27 * pow(82, -1, BN254_Q) % BN254_Q, -3 * pow(82, -1, BN254_Q) % BN254_Q)  # 3 (9 - u) / 82
 
 
 def mont_block(prefix, p, n, b, gx, gy):
@@ -95,9 +102,10 @@ def mont_block(prefix, p, n, b, gx, gy):
     return "\n".join(out)
 
 
-def fp2_block(prefix, p, n, b, gx, gy):
+def fp2_block(prefix, p, n, b, gx, gy, b3=False):
     """The generator of a curve y^2 = x^3 + b over Fp2 = Fp[u]/(u^2 + 1), b and the coordinates as
-    (c0, c1): 2n limbs per coordinate, the Montgomery c0 (R = 2^(32 n)) then c1."""
+    (c0, c1): 2n limbs per coordinate, the Montgomery c0 (R = 2^(32 n)) then c1; with b3, also 3b
+    (for twists where multiplying by 3b takes an Fp2 product rather than additions)."""
     def mul(x, y):
         return ((x[0] * y[0] - x[1] * y[1]) % p, (x[0] * y[1] + x[1] * y[0]) % p)
     x3 = mul(mul(gx, gx), gx)
@@ -106,8 +114,11 @@ def fp2_block(prefix, p, n, b, gx, gy):
 
     def mont(v):
         return v[0] * R % p + (v[1] * R % p << (32 * n))
-    return "\n".join([f"// ---- {prefix}: generator of y^2 = x^3 + ({b[0]} + {b[1]} u) over Fp2, p = 0x{p:x}",
-                      table(f"{prefix}_GX", mont(gx), 2 * n), table(f"{prefix}_GY", mont(gy), 2 * n)])
+    out = [f"// ---- {prefix}: generator of y^2 = x^3 + ({b[0]} + {b[1]} u) over Fp2, p = 0x{p:x}",
+           table(f"{prefix}_GX", mont(gx), 2 * n), table(f"{prefix}_GY", mont(gy), 2 * n)]
+    if b3:
+        out.append(table(f"{prefix}_B3", mont((3 * b[0] % p, 3 * b[1] % p)), 2 * n))
+    return "\n".join(out)
 
 
 L25519 = 2**252 + 27742317777372353535851937790883648493  # order of the ristretto255 group
@@ -150,6 +161,7 @@ def main():
     parts.append(mont_block("GK", BN254_R, 8, -17, 1, sqrt_mod(-16 % BN254_R, BN254_R)))
     parts.append(mont_block("BLS", BLS_Q, 12, 4, BLS_GX, BLS_GY))
     parts.append(fp2_block("BLS2", BLS_Q, 12, (4, 4), BLS2_GX, BLS2_GY))
+    parts.append(fp2_block("BN2", BN254_Q, 8, BN2_B, BN2_GX, BN2_GY, b3=True))
     parts.append(scalar_block("SC25", L25519, 8))
     parts.append("}  // namespace b200")
     here = os.path.dirname(os.path.abspath(__file__))

@@ -167,6 +167,18 @@ struct b200_bls12_381_g2 { uint64_t X[12]; uint64_t Y[12]; uint8_t infinity; };
 struct b200_bls12_381_g2_p2 { uint64_t X[12]; uint64_t Y[12]; uint64_t Z[12]; };
 struct b200_bls12_381_g2_compressed { uint8_t g2_bytes[96]; };
 
+/* bn254 G2 (y^2 = x^3 + 3 / (9 + u) over Fp2 = Fp[u]/(u^2 + 1), the twist of EIP-197, generator as
+ * there), accepted wherever curve 4 is. It has no counterpart in the reference either. Coordinates are
+ * Fp2 elements c0 + c1 u as 4 Montgomery u64 limbs (R = 2^256) of c0, then 4 of c1 (EIP-197 and
+ * snarkjs list c1 first: swap them on the way in and out). Commitment generators (and the affine
+ * synthetic generators) are b200_bn254_g2, 136 bytes each; handle generators and fixed-MSM results are
+ * b200_bn254_g2_p2 (projective, identity Z = 0); commitments are b200_bn254_g2 as well, uncompressed
+ * affine Montgomery coordinates as for bn254 G1 (identity {0, 1, infinity = 1}). b200_field_op's
+ * field 7 is this Fp2. */
+#define B200_CURVE_BN254_G2 5
+struct b200_bn254_g2 { uint64_t X[8]; uint64_t Y[8]; uint8_t infinity; };
+struct b200_bn254_g2_p2 { uint64_t X[8]; uint64_t Y[8]; uint64_t Z[8]; };
+
 /* Bind the calling thread / library to a CUDA device before sxt_init (default: current device). */
 void b200_set_device(int device);
 /* Number of kernels this library has launched so far in this process. */
@@ -303,14 +315,15 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
  * b[i]). Operands and results are little-endian u32 limbs. Fields: 0 curve25519 Fp (8 limbs, loosely
  * reduced: any value below 2^256), 1 bls12-381 Fp (12), 2 bn254 Fp (8), 3 grumpkin Fp (8), 4 the
  * ristretto255 scalars mod l (8), 5 curve25519 Fp lane-sliced over 10 lanes (10 limbs of radix
- * 2^25.5), 6 bls12-381 Fp2 (24: c0 then c1). Fields 1-4 and 6 hold Montgomery residues. Ops: 0 add,
- * 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref, 6 sqr (fields 0-4, 6); field 0: 7 mul_lat, 8 canonical,
- * 9 is_negative (1 limb out), 10 invert, 11 pow22523, 12 from_radix51 (10 limbs in: 5 x u64),
- * 13 to_radix51 (10 limbs out), 14 sqrt_ratio_m1 (a = u, b = v; out: x, then the was-square flag);
- * fields 1-4 and 6: 10 invert, 15 invert_eea, 16 from_mont, 17 to_mont, 18 lexicographically_largest
- * (1 limb out; field 6: the zcash rule, c1 decides unless it is 0); field 5: 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p, 22 slice (8 limbs in), 23 gather (8
- * limbs out). b is read only by binary ops (add, sub, mul, mul_ref, mul_lat, sqrt_ratio_m1, sub2p,
- * sub4p). Host pointers; synchronises. Returns 0, or ~0u when the field does not offer op. */
+ * 2^25.5), 6 bls12-381 Fp2 (24: c0 then c1), 7 bn254 Fp2 (16: c0 then c1). Fields 1-4, 6 and 7
+ * hold Montgomery residues. Ops: 0 add, 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref, 6 sqr (fields 0-4,
+ * 6, 7); field 0: 7 mul_lat, 8 canonical, 9 is_negative (1 limb out), 10 invert, 11 pow22523,
+ * 12 from_radix51 (10 limbs in: 5 x u64), 13 to_radix51 (10 limbs out), 14 sqrt_ratio_m1 (a = u,
+ * b = v; out: x, then the was-square flag); fields 1-4, 6 and 7: 10 invert, 15 invert_eea,
+ * 16 from_mont, 17 to_mont, 18 lexicographically_largest (1 limb out; fields 6 and 7: the zcash rule,
+ * c1 decides unless it is 0); field 5: 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p,
+ * 22 slice (8 limbs in), 23 gather (8 limbs out). b is read only by binary ops (add, sub, mul,
+ * mul_ref, mul_lat, sqrt_ratio_m1, sub2p, sub4p). Host pointers; synchronises. Returns 0, or ~0u when the field does not offer op. */
 unsigned b200_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
                        const uint32_t* b, uint32_t* out);
 /* Self-test of the binned bucket sort: sorts the (term, window) entries of the device-resident
