@@ -51,6 +51,7 @@ B200_SYMBOLS = [
     "b200_compute_pedersen_commitments_with_offsets", "b200_commit_device_with_offsets",
     "b200_multiexp_handle_add_partition_table", "b200_multiexp_handle_partition_window",
     "b200_curve25519_prove_inner_products", "b200_curve25519_verify_inner_products",
+    "b200_multi_pairing", "b200_multi_pairing_device",
 ]
 
 
@@ -346,11 +347,12 @@ def selftest_lane_arithmetic(warps=64, seed=1):
 
 
 # b200_field_op: limbs per element of each field, and the operation codes
-FIELD_LIMBS = {0: 8, 1: 12, 2: 8, 3: 8, 4: 8, 5: 10, 6: 24, 7: 16}
+FIELD_LIMBS = {0: 8, 1: 12, 2: 8, 3: 8, 4: 8, 5: 10, 6: 24, 7: 16, 8: 144, 9: 96}
 FIELD_OPS = {name: code for code, name in enumerate([
     "add", "sub", "neg", "dbl", "mul", "mul_ref", "sqr", "mul_lat", "canonical", "is_negative",
     "invert", "pow22523", "from_radix51", "to_radix51", "sqrt_ratio_m1", "invert_eea", "from_mont",
-    "to_mont", "lexicographically_largest", "carry1", "sub2p", "sub4p", "slice", "gather"])}
+    "to_mont", "lexicographically_largest", "carry1", "sub2p", "sub4p", "slice", "gather",
+    "frobenius", "cyclotomic_sqr", "final_exp"])}
 _BINARY_OPS = {"add", "sub", "mul", "mul_ref", "mul_lat", "sqrt_ratio_m1", "sub2p", "sub4p"}
 
 
@@ -607,3 +609,42 @@ def call_verify_inner_products(entry, transcripts, b_list, products, a_commits, 
           _ptr(np.ascontiguousarray(a_commits, np.uint8)), _ptr(np.ascontiguousarray(lrs[0])),
           _ptr(np.ascontiguousarray(lrs[1])), _ptr(np.ascontiguousarray(ap_values, np.uint8)))
     return results[:P]
+
+
+# ---- pairing products ----------------------------------------------------------------------------
+# bytes of one GT element (b200_bls12_381_gt / b200_bn254_gt) per G1 curve id, and the G2 curve paired
+# with it
+GT_BYTES = {SXT_CURVE_BLS_381: 576, SXT_CURVE_BN_254: 384}
+PAIRING_G2 = {SXT_CURVE_BLS_381: B200_CURVE_BLS12_381_G2, SXT_CURVE_BN_254: B200_CURVE_BN254_G2}
+
+
+def call_multi_pairing(entry, curve_id, g1_p2, g2_p2, lengths):
+    """Runs a b200_multi_pairing-shaped entry on host arrays: g1_p2 / g2_p2 uint8 [n, projective
+    struct bytes] of curve_id's G1 and G2, lengths the pairs of each product (summing to n). Returns
+    uint8 [num_products, GT_BYTES[curve_id]]."""
+    if curve_id not in GT_BYTES:
+        raise ValueError(f"no pairing for curve {curve_id}")
+    lengths = np.ascontiguousarray(lengths, dtype=np.uint32).reshape(-1)
+    n = int(lengths.sum(dtype=np.uint64))
+    g1 = np.ascontiguousarray(g1_p2, dtype=np.uint8).reshape(-1, CURVE_SIZES[curve_id][0])
+    g2 = np.ascontiguousarray(g2_p2, dtype=np.uint8).reshape(-1, CURVE_SIZES[PAIRING_G2[curve_id]][0])
+    if g1.shape[0] != n or g2.shape[0] != n:
+        raise ValueError(f"g1_p2 and g2_p2 must hold sum(lengths) = {n} points each")
+    out = np.zeros((lengths.size, GT_BYTES[curve_id]), dtype=np.uint8)
+    entry(C.c_uint(curve_id), _ptr(out), C.c_uint32(lengths.size), _ptr(lengths),
+          _ptr(g1 if n else None), _ptr(g2 if n else None))
+    return out
+
+
+def multi_pairing(curve_id, g1_p2, g2_p2, lengths):
+    """b200_multi_pairing: out[k] = prod e(g1[i], g2[i]) over product k's lengths[k] consecutive
+    pairs, as GT ABI bytes (call_multi_pairing)."""
+    return call_multi_pairing(lib().b200_multi_pairing, curve_id, g1_p2, g2_p2, lengths)
+
+
+def multi_pairing_device(curve_id, out_ptr, lengths, g1_ptr, g2_ptr):
+    """b200_multi_pairing_device: device pointers, lengths a host sequence; enqueued on the library
+    stream."""
+    lengths = np.ascontiguousarray(lengths, dtype=np.uint32).reshape(-1)
+    lib().b200_multi_pairing_device(C.c_uint(curve_id), C.c_void_p(out_ptr), C.c_uint32(lengths.size),
+                                    _ptr(lengths), C.c_void_p(g1_ptr), C.c_void_p(g2_ptr))

@@ -1482,6 +1482,49 @@ unsigned b200_multiexp_handle_partition_window(const struct sxt_multiexp_handle*
   const HandleSet* hs = handle_of(handle);
   return hs->shards.empty() ? 0u : hs->shards[0]->ptable_w;
 }
+namespace {
+// the number of pairs of a b200_multi_pairing* call, after its checks
+uint64_t check_multi_pairing(unsigned curve_id, const void* out, uint32_t num_products,
+                             const uint32_t* lengths, const void* g1, const void* g2) {
+  B200_REQUIRE(curve_id == SXT_CURVE_BLS_381 || curve_id == SXT_CURVE_BN_254,
+               "pairings are defined for curve ids 1 (bls12-381) and 2 (bn254) only");
+  B200_REQUIRE(num_products == 0 || (out != nullptr && lengths != nullptr),
+               "out / lengths must not be null");
+  uint64_t total = 0;
+  for (uint32_t k = 0; k < num_products; ++k)
+    total += lengths[k];
+  B200_REQUIRE(total < (1ull << 31), "2^31 or more pairs in one call");
+  B200_REQUIRE(total == 0 || (g1 != nullptr && g2 != nullptr), "g1 / g2 must not be null");
+  return total;
+}
+}  // namespace
+
+void b200_multi_pairing(unsigned curve_id, void* out, uint32_t num_products,
+                        const uint32_t* lengths, const void* g1, const void* g2) {
+  const Entry entry("b200_multi_pairing");
+  const uint64_t n = check_multi_pairing(curve_id, out, num_products, lengths, g1, g2);
+  if (num_products == 0)
+    return;
+  cudaStream_t s = g_state.stream;
+  const size_t b1 = curve_vtable(curve_id).abi_proj_bytes;
+  const size_t b2 = curve_vtable(curve_id == SXT_CURVE_BLS_381 ? B200_CURVE_BLS12_381_G2
+                                                               : B200_CURVE_BN254_G2).abi_proj_bytes;
+  const size_t gt = curve_id == SXT_CURVE_BLS_381 ? sizeof(b200_bls12_381_gt) : sizeof(b200_bn254_gt);
+  DevBuf<unsigned char> d1(n * b1, s), d2(n * b2, s), dout(num_products * gt, s);
+  copy_h2d(d1.p, g1, n * b1, s);
+  copy_h2d(d2.p, g2, n * b2, s);
+  multi_pairing(ctx(), curve_id, dout.p, num_products, lengths, d1.p, d2.p);
+  copy_d2h(out, dout.p, num_products * gt, s);
+  stream_sync(s);
+}
+void b200_multi_pairing_device(unsigned curve_id, void* out, uint32_t num_products,
+                               const uint32_t* lengths, const void* g1, const void* g2) {
+  const Entry entry("b200_multi_pairing_device");
+  check_multi_pairing(curve_id, out, num_products, lengths, g1, g2);
+  if (num_products == 0)
+    return;
+  multi_pairing(ctx(), curve_id, out, num_products, lengths, g1, g2);
+}
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   const Entry entry("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);

@@ -335,6 +335,11 @@ unsigned field_op_bls12381_g2(const EngineCtx& ctx, unsigned op, uint64_t n, con
                               const uint32_t* b, uint32_t* out);
 unsigned field_op_bn254_g2(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
                            const uint32_t* b, uint32_t* out);
+// the Fp12 of each pairing (pairing.cuh; fields 8 and 9)
+unsigned field_op_bls12381_gt(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                              const uint32_t* b, uint32_t* out);
+unsigned field_op_bn254_gt(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
+                           const uint32_t* b, uint32_t* out);
 inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
                          const uint32_t* a, const uint32_t* b, uint32_t* out) {
   switch (field) {
@@ -343,8 +348,25 @@ inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint
   case 3: return field_op_grumpkin(ctx, op, n, a, b, out);
   case 6: return field_op_bls12381_g2(ctx, op, n, a, b, out);
   case 7: return field_op_bn254_g2(ctx, op, n, a, b, out);
+  case 8: return field_op_bls12381_gt(ctx, op, n, a, b, out);
+  case 9: return field_op_bn254_gt(ctx, op, n, a, b, out);
   default: return field_op_ed25519(ctx, field, op, n, a, b, out);
   }
+}
+
+// pairing products (pairing.cuh; b200_multi_pairing_device's contract, curve_id 1 or 2 checked by the
+// caller): out[k] = prod e(g1[i], g2[i]) over product k's lengths[k] consecutive pairs
+void multi_pairing_bls12381(const EngineCtx& ctx, void* out, uint32_t num_products,
+                            const uint32_t* lengths, const void* g1, const void* g2);
+void multi_pairing_bn254(const EngineCtx& ctx, void* out, uint32_t num_products,
+                         const uint32_t* lengths, const void* g1, const void* g2);
+inline void multi_pairing(const EngineCtx& ctx, unsigned curve_id, void* out,
+                          uint32_t num_products, const uint32_t* lengths, const void* g1,
+                          const void* g2) {
+  if (curve_id == SXT_CURVE_BLS_381)
+    multi_pairing_bls12381(ctx, out, num_products, lengths, g1, g2);
+  else
+    multi_pairing_bn254(ctx, out, num_products, lengths, g1, g2);
 }
 
 // built-in ristretto generators g(first .. first+n) into the device generator layout

@@ -18,6 +18,7 @@ enum : u32 {
   kOpFromRadix51, kOpToRadix51, kOpSqrtRatioM1,                      // pow22523: lane too)
   kOpInvertEea, kOpFromMont, kOpToMont, kOpLexLargest,               // Montgomery fields
   kOpCarry1, kOpSub2p, kOpSub4p, kOpSlice, kOpGather,                // lane-sliced F25519
+  kOpFrobenius, kOpCyclotomicSqr, kOpFinalExp,                       // Fp12 (pairing.cuh)
 };
 
 // u32 limbs per element of operand a, operand b (0 = unary) and the result; out = 0: not offered

@@ -121,6 +121,74 @@ def fp2_block(prefix, p, n, b, gx, gy, b3=False):
     return "\n".join(out)
 
 
+BLS_R = 0x73eda753299d7d483339d80809a1d80553bda402fffe5bfeffffffff00000001
+# the curve parameters x of the two pairing-friendly families (bls12-381: x < 0; bn254: x > 0)
+BLS_X = -0xd201000000010000
+BN_X = 0x44e992b44a6909f1
+
+
+def tower_block(prefix, p, r, n, xi0, x):
+    """Constants of the pairing tower Fp6 = Fp2[v] / (v^3 - xi), Fp12 = Fp6[w] / (w^2 - v) over
+    Fp2 = Fp[u] / (u^2 + 1), xi = xi0 + u (pairing.cuh): the Frobenius coefficients
+    gamma_{k,i} = xi^(i (p^k - 1) / 6) of w^i (k = 1..3, i = 1..5, flattened as ((k-1) 5 + i-1) 2n
+    limbs, Montgomery c0 then c1), 1/2, the Miller loop count, |x|, the hard part of the final
+    exponentiation and, for bn254, the twist Frobenius constants of pi(Q)."""
+    def mul(a, b):
+        return ((a[0] * b[0] - a[1] * b[1]) % p, (a[0] * b[1] + a[1] * b[0]) % p)
+
+    def pw(a, e):
+        acc = (1, 0)
+        for bit in bin(e)[2:]:
+            acc = mul(acc, acc)
+            if bit == "1":
+                acc = mul(acc, a)
+        return acc
+    R = 1 << (32 * n)
+
+    def mont(v):
+        return v[0] * R % p + (v[1] * R % p << (32 * n))
+    xi = (xi0, 1)
+    assert p % 4 == 3 and (p - 1) % 6 == 0
+    # the tower is a field: xi is neither a square nor a cube in Fp2
+    assert pw(xi, (p * p - 1) // 2) != (1, 0) and pw(xi, (p * p - 1) // 3) != (1, 0)
+    flat = 0
+    for k in (1, 2, 3):
+        for i in range(1, 6):
+            g = pw(xi, i * (p ** k - 1) // 6)
+            if k == 2:  # the p^2 coefficients lie in Fp and are sixth roots of unity
+                assert g[1] == 0 and pw(g, 6) == (1, 0)
+            flat |= mont(g) << (64 * n * ((k - 1) * 5 + i - 1))
+    loop = abs(x) if x < 0 else 6 * x + 2  # bls12-381: the ate loop |x|; bn254: the optimal ate 6x + 2
+    hard = (p ** 4 - p ** 2 + 1) // r
+    assert (p ** 4 - p ** 2 + 1) % r == 0
+    if x < 0:  # bls12-381: lambda_3 = (x - 1)^2 / 3, lambda_2 = lambda_3 x, lambda_1 = lambda_2 x - lambda_3,
+        assert (x - 1) ** 2 % 3 == 0  # lambda_0 = lambda_1 x + 1
+        l3 = (x - 1) ** 2 // 3
+        l2 = l3 * x
+        l1 = l2 * x - l3
+        l0 = l1 * x + 1
+    else:  # bn254 (Devegili-Scott-Dahab)
+        l3, l2 = 1, 6 * x * x + 1
+        l1 = -36 * x ** 3 - 18 * x ** 2 - 12 * x + 1
+        l0 = -36 * x ** 3 - 30 * x ** 2 - 18 * x - 2
+    assert l0 + l1 * p + l2 * p ** 2 + l3 * p ** 3 == hard
+    out = [f"// ---- {prefix}: pairing tower over Fp2 of p = 0x{p:x}, xi = {xi0} + u, x = {x}",
+           f"constexpr u32 {prefix}_XI0 = {xi0}u;  // xi = {xi0} + u",
+           table(f"{prefix}_FROB", flat, 30 * n),
+           table(f"{prefix}_TWO_INV", (p + 1) // 2 * R % p, n),
+           f"constexpr u64 {prefix}_LOOP_LO = 0x{loop & (2**64 - 1):016x}ull;  // Miller loop count",
+           f"constexpr u64 {prefix}_LOOP_HI = 0x{loop >> 64:x}ull;",
+           f"constexpr int {prefix}_LOOP_BITS = {loop.bit_length()};",
+           f"constexpr u64 {prefix}_X_ABS = 0x{abs(x):016x}ull;",
+           f"constexpr bool {prefix}_X_NEG = {'true' if x < 0 else 'false'};",
+           f"constexpr u64 {prefix}_LAMBDA3_LO = 0x{l3 & (2**64 - 1):016x}ull;  // hard part, lambda_3",
+           f"constexpr u64 {prefix}_LAMBDA3_HI = 0x{l3 >> 64:016x}ull;"]
+    if x > 0:  # pi(x', y') = (conj(x') xi^((p-1)/3), conj(y') xi^((p-1)/2)) on the D-type twist
+        out.append(table(f"{prefix}_TWIST_FROB_X", mont(pw(xi, (p - 1) // 3)), 2 * n))
+        out.append(table(f"{prefix}_TWIST_FROB_Y", mont(pw(xi, (p - 1) // 2)), 2 * n))
+    return "\n".join(out)
+
+
 L25519 = 2**252 + 27742317777372353535851937790883648493  # order of the ristretto255 group
 
 
@@ -163,6 +231,8 @@ def main():
     parts.append(fp2_block("BLS2", BLS_Q, 12, (4, 4), BLS2_GX, BLS2_GY))
     parts.append(fp2_block("BN2", BN254_Q, 8, BN2_B, BN2_GX, BN2_GY, b3=True))
     parts.append(scalar_block("SC25", L25519, 8))
+    parts.append(tower_block("BLS12", BLS_Q, BLS_R, 12, 1, BLS_X))
+    parts.append(tower_block("BN12", BN254_Q, BN254_R, 8, 9, BN_X))
     parts.append("}  // namespace b200")
     here = os.path.dirname(os.path.abspath(__file__))
     path, text = os.path.join(here, "constants.cuh"), "\n".join(parts) + "\n"

@@ -179,6 +179,14 @@ struct b200_bls12_381_g2_compressed { uint8_t g2_bytes[96]; };
 struct b200_bn254_g2 { uint64_t X[8]; uint64_t Y[8]; uint8_t infinity; };
 struct b200_bn254_g2_p2 { uint64_t X[8]; uint64_t Y[8]; uint64_t Z[8]; };
 
+/* GT = the order-r subgroup of Fp12*, Fp12 = Fp6[w]/(w^2 - v), Fp6 = Fp2[v]/(v^3 - xi), Fp2 as for G2
+ * (xi = 1 + u for bls12-381, 9 + u for bn254). An element is 12 Fp components in the order
+ * c0.b0.a0, c0.b0.a1, c0.b1.a0, ..., c1.b2.a1 (c: over w, b: over v, a: over u), each as Montgomery
+ * u64 limbs (R = 2^384 / 2^256), like the curves' coordinates. b200_field_op's fields 8 and 9 are these
+ * two Fp12s. */
+struct b200_bls12_381_gt { uint64_t c[72]; };   /* 576 bytes */
+struct b200_bn254_gt     { uint64_t c[48]; };   /* 384 bytes */
+
 /* Bind the calling thread / library to a CUDA device before sxt_init (default: current device). */
 void b200_set_device(int device);
 /* Number of kernels this library has launched so far in this process. */
@@ -307,6 +315,23 @@ uint32_t b200_curve25519_verify_inner_products(
     const struct sxt_ristretto255_compressed* l_vectors /* sum k_p */,
     const struct sxt_ristretto255_compressed* r_vectors /* sum k_p */,
     const struct sxt_curve25519_scalar* ap_values);
+/* out[k] = prod_{i in product k} e(g1[i], g2[i]), for k < num_products. curve_id is
+ * SXT_CURVE_BLS_381 or SXT_CURVE_BN_254, naming the G1 curve. Its G2 (curve 4 / 5) is implied.
+ * Product k owns lengths[k] consecutive pairs, starting at the sum of the earlier lengths.
+ * g1 holds sxt_bls12_381_g1_p2 / sxt_bn254_g1_p2 structs and g2 holds b200_*_g2_p2 structs:
+ * projective, (x, y) = (X/Z, Y/Z), which is how the fixed-base calls write their results.
+ * A pair with an identity (Z = 0) on either side contributes 1. An empty product is 1.
+ * e(P, Q) = f^((p^12 - 1)/r) with exactly this exponent: bls12-381 f = conj(f_{|x|,Q}(P)) (the ate
+ * Miller function, x = -0xd201000000010000); bn254 f = f_{6x+2,Q}(P) l_{T,pi(Q)}(P) l_{T+pi(Q),-pi^2(Q)}(P)
+ * (optimal ate, x = 0x44e992b44a6909f1, T = [6x+2]Q). Points are not checked to be on their curves or
+ * in the order-r subgroups. Aborts for another curve_id, null pointers where there are pairs, and 2^31
+ * or more pairs in total. Host pointers; synchronises. */
+void b200_multi_pairing(unsigned curve_id, void* out, uint32_t num_products,
+                        const uint32_t* lengths, const void* g1, const void* g2);
+/* as above, but out, g1 and g2 are DEVICE pointers and lengths is a host array; enqueued on the
+ * library stream, returns without synchronising */
+void b200_multi_pairing_device(unsigned curve_id, void* out, uint32_t num_products,
+                               const uint32_t* lengths, const void* g1, const void* g2);
 /* Self-test of the warp-cooperative (lane-sliced) field arithmetic of the tail kernels against the
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
@@ -315,9 +340,12 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
  * b[i]). Operands and results are little-endian u32 limbs. Fields: 0 curve25519 Fp (8 limbs, loosely
  * reduced: any value below 2^256), 1 bls12-381 Fp (12), 2 bn254 Fp (8), 3 grumpkin Fp (8), 4 the
  * ristretto255 scalars mod l (8), 5 curve25519 Fp lane-sliced over 10 lanes (10 limbs of radix
- * 2^25.5), 6 bls12-381 Fp2 (24: c0 then c1), 7 bn254 Fp2 (16: c0 then c1). Fields 1-4, 6 and 7
- * hold Montgomery residues. Ops: 0 add, 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref, 6 sqr (fields 0-4,
- * 6, 7); field 0: 7 mul_lat, 8 canonical, 9 is_negative (1 limb out), 10 invert, 11 pow22523,
+ * 2^25.5), 6 bls12-381 Fp2 (24: c0 then c1), 7 bn254 Fp2 (16: c0 then c1), 8 bls12-381 Fp12 (144)
+ * and 9 bn254 Fp12 (96), in the GT layout above. Fields 1-4 and 6-9 hold Montgomery residues.
+ * Ops: 0 add, 1 sub, 2 neg, 3 dbl, 4 mul, 5 mul_ref, 6 sqr (fields 0-4, 6, 7); fields 8 and 9: 0 add,
+ * 1 sub, 2 neg, 4 mul, 6 sqr, 10 invert, 24 frobenius (a^p), 25 cyclotomic_sqr (a must satisfy
+ * a^(p^6 + 1) = 1), 26 final_exp (a^((p^12 - 1)/r)); field 0: 7 mul_lat, 8 canonical, 9 is_negative
+ * (1 limb out), 10 invert, 11 pow22523,
  * 12 from_radix51 (10 limbs in: 5 x u64), 13 to_radix51 (10 limbs out), 14 sqrt_ratio_m1 (a = u,
  * b = v; out: x, then the was-square flag); fields 1-4, 6 and 7: 10 invert, 15 invert_eea,
  * 16 from_mont, 17 to_mont, 18 lexicographically_largest (1 limb out; fields 6 and 7: the zcash rule,
