@@ -52,6 +52,8 @@ B200_SYMBOLS = [
     "b200_multiexp_handle_add_partition_table", "b200_multiexp_handle_partition_window",
     "b200_curve25519_prove_inner_products", "b200_curve25519_verify_inner_products",
     "b200_multi_pairing", "b200_multi_pairing_device",
+    "b200_check_points", "b200_decode_points", "b200_check_points_device",
+    "b200_decode_points_device",
 ]
 
 
@@ -352,7 +354,7 @@ FIELD_OPS = {name: code for code, name in enumerate([
     "add", "sub", "neg", "dbl", "mul", "mul_ref", "sqr", "mul_lat", "canonical", "is_negative",
     "invert", "pow22523", "from_radix51", "to_radix51", "sqrt_ratio_m1", "invert_eea", "from_mont",
     "to_mont", "lexicographically_largest", "carry1", "sub2p", "sub4p", "slice", "gather",
-    "frobenius", "cyclotomic_sqr", "final_exp"])}
+    "frobenius", "cyclotomic_sqr", "final_exp", "sqrt"])}
 _BINARY_OPS = {"add", "sub", "mul", "mul_ref", "mul_lat", "sqrt_ratio_m1", "sub2p", "sub4p"}
 
 
@@ -361,7 +363,7 @@ def field_op_shape(field, op):
     n = FIELD_LIMBS[field]
     a = {"from_radix51": 10, "slice": 8}.get(op, n)
     out = {"is_negative": 1, "lexicographically_largest": 1, "to_radix51": 10,
-           "sqrt_ratio_m1": n + 1, "gather": 8}.get(op, n)
+           "sqrt_ratio_m1": n + 1, "sqrt": n + 1, "gather": 8}.get(op, n)
     return a, (n if op in _BINARY_OPS else 0), out
 
 
@@ -648,3 +650,66 @@ def multi_pairing_device(curve_id, out_ptr, lengths, g1_ptr, g2_ptr):
     lengths = np.ascontiguousarray(lengths, dtype=np.uint32).reshape(-1)
     lib().b200_multi_pairing_device(C.c_uint(curve_id), C.c_void_p(out_ptr), C.c_uint32(lengths.size),
                                     _ptr(lengths), C.c_void_p(g1_ptr), C.c_void_p(g2_ptr))
+
+
+# ---- point checks and decoding -------------------------------------------------------------------
+POINT_CURVES = (1, 2, 3, 4, 5)
+
+
+def _point_rows(curve_id, data, column):
+    if curve_id not in POINT_CURVES:
+        raise ValueError(f"no point checks for curve {curve_id}")
+    width = CURVE_SIZES[curve_id][column]
+    return np.ascontiguousarray(data, dtype=np.uint8).reshape(-1, width)
+
+
+def call_check_points(entry, curve_id, p2):
+    """Runs a b200_check_points-shaped entry on host *_p2 structs (uint8 [n, projective bytes]).
+    Returns (valid uint8 [n], the entry's count of valid points)."""
+    p2 = _point_rows(curve_id, p2, 0)
+    valid = np.zeros(p2.shape[0], dtype=np.uint8)
+    entry.restype = C.c_uint64
+    count = entry(C.c_uint(curve_id), _ptr(valid), _ptr(p2 if p2.shape[0] else None),
+                  C.c_uint64(p2.shape[0]))
+    return valid, int(count)
+
+
+def call_decode_points(entry, curve_id, encoded):
+    """Runs a b200_decode_points-shaped entry on host commitments (uint8 [n, commitment bytes]).
+    Returns (p2 uint8 [n, projective bytes], valid uint8 [n], the entry's count of valid points)."""
+    encoded = _point_rows(curve_id, encoded, 2)
+    n = encoded.shape[0]
+    out = np.zeros((n, CURVE_SIZES[curve_id][0]), dtype=np.uint8)
+    valid = np.zeros(n, dtype=np.uint8)
+    entry.restype = C.c_uint64
+    count = entry(C.c_uint(curve_id), _ptr(out if n else None), _ptr(valid if n else None),
+                  _ptr(encoded if n else None), C.c_uint64(n))
+    return out, valid, int(count)
+
+
+def check_points(curve_id, p2):
+    """b200_check_points: valid uint8 [n], 1 where p2[i] (the curve's projective struct) is a point
+    of the order-r group. Compare valid.sum() with n before trusting the points."""
+    return call_check_points(lib().b200_check_points, curve_id, p2)[0]
+
+
+def decode_points(curve_id, encoded):
+    """b200_decode_points: (p2 uint8 [n, projective bytes], valid uint8 [n]) from commitments in
+    the curve's encoding. An invalid input decodes to the identity with valid 0."""
+    return call_decode_points(lib().b200_decode_points, curve_id, encoded)[:2]
+
+
+def check_points_device(curve_id, valid_ptr, points_ptr, n):
+    """b200_check_points_device: device pointers; enqueued on the library stream."""
+    if curve_id not in POINT_CURVES:
+        raise ValueError(f"no point checks for curve {curve_id}")
+    lib().b200_check_points_device(C.c_uint(curve_id), C.c_void_p(valid_ptr),
+                                   C.c_void_p(points_ptr), C.c_uint64(n))
+
+
+def decode_points_device(curve_id, out_ptr, valid_ptr, encoded_ptr, n):
+    """b200_decode_points_device: device pointers; enqueued on the library stream."""
+    if curve_id not in POINT_CURVES:
+        raise ValueError(f"no point checks for curve {curve_id}")
+    lib().b200_decode_points_device(C.c_uint(curve_id), C.c_void_p(out_ptr), C.c_void_p(valid_ptr),
+                                    C.c_void_p(encoded_ptr), C.c_uint64(n))

@@ -14,7 +14,8 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", "-O3"] + ARCH + ["-lineinfo",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC"]
 UNITS = ["api.cu", "curve_ed25519.cu", "curve_bls12381.cu", "curve_bn254.cu", "curve_grumpkin.cu",
-         "curve_bls12381_g2.cu", "curve_bn254_g2.cu", "pairing_bls12381.cu", "pairing_bn254.cu"]
+         "curve_bls12381_g2.cu", "curve_bn254_g2.cu", "pairing_bls12381.cu", "pairing_bn254.cu",
+         "points_bls12381.cu", "points_bn254.cu"]
 
 
 def _newer(target, sources):
@@ -54,8 +55,8 @@ def build_product(verbose=False):
 
 
 def build_emul():
-    """CPU emulation harness (test infrastructure): the per-curve and pairing units of the product
-    and the harness's own sources (tests/emul/*.cpp) compiled as host C++ (-DB200_EMULATE,
+    """CPU emulation harness (test infrastructure): the per-curve, pairing and point units of the
+    product and the harness's own sources (tests/emul/*.cpp) compiled as host C++ (-DB200_EMULATE,
     tests/emul/emul_prefix.h force-included), in parallel."""
     edir = os.path.join(ROOT, "tests", "emul")
     out = os.path.join(edir, "libb200_emul.so")
@@ -65,7 +66,7 @@ def build_emul():
     flags = ["g++", "-std=c++17", "-O1", "-DB200_EMULATE", "-fPIC", "-w", "-include", prefix]
     jobs, objs = [], []
     harness = sorted(f for f in os.listdir(edir) if f.endswith(".cpp"))
-    srcs = [os.path.join(CSRC, u) for u in UNITS if u.startswith(("curve_", "pairing_"))] + \
+    srcs = [os.path.join(CSRC, u) for u in UNITS if u.startswith(("curve_", "pairing_", "points_"))] + \
         [os.path.join(edir, f) for f in harness]
     for src in srcs:
         u = os.path.basename(src)

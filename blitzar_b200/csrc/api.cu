@@ -1525,6 +1525,63 @@ void b200_multi_pairing_device(unsigned curve_id, void* out, uint32_t num_produc
     return;
   multi_pairing(ctx(), curve_id, out, num_products, lengths, g1, g2);
 }
+namespace {
+// the checks of the b200_check_points* and b200_decode_points* calls
+void check_points_call(unsigned curve_id, bool pointers_set, uint64_t n) {
+  B200_REQUIRE(curve_id >= SXT_CURVE_BLS_381 && curve_id <= B200_CURVE_BN254_G2,
+               "point checks are defined for curve ids 1-5 (a ristretto255 encoding is checked by "
+               "decoding it)");
+  B200_REQUIRE(n == 0 || pointers_set, "valid / points must not be null");
+}
+uint64_t count_valid(const uint8_t* valid, uint64_t n) {
+  uint64_t count = 0;
+  for (uint64_t i = 0; i < n; ++i)
+    count += valid[i] != 0;
+  return count;
+}
+}  // namespace
+
+uint64_t b200_check_points(unsigned curve_id, uint8_t* valid, const void* points, uint64_t n) {
+  const Entry entry("b200_check_points");
+  check_points_call(curve_id, valid != nullptr && points != nullptr, n);
+  if (n == 0)
+    return 0;
+  cudaStream_t s = g_state.stream;
+  const size_t bytes = curve_vtable(curve_id).abi_proj_bytes;
+  DevBuf<unsigned char> dp(n * bytes, s), dv(n, s);
+  copy_h2d(dp.p, points, n * bytes, s);
+  check_points(ctx(), curve_id, dv.p, dp.p, n);
+  copy_d2h(valid, dv.p, n, s);
+  stream_sync(s);
+  return count_valid(valid, n);
+}
+uint64_t b200_decode_points(unsigned curve_id, void* out_p2, uint8_t* valid, const void* encoded,
+                            uint64_t n) {
+  const Entry entry("b200_decode_points");
+  check_points_call(curve_id, out_p2 != nullptr && valid != nullptr && encoded != nullptr, n);
+  if (n == 0)
+    return 0;
+  cudaStream_t s = g_state.stream;
+  const CurveVTable& vt = curve_vtable(curve_id);
+  DevBuf<unsigned char> de(n * vt.abi_commit_bytes, s), dout(n * vt.abi_proj_bytes, s), dv(n, s);
+  copy_h2d(de.p, encoded, n * vt.abi_commit_bytes, s);
+  decode_points(ctx(), curve_id, dout.p, dv.p, de.p, n);
+  copy_d2h(out_p2, dout.p, n * vt.abi_proj_bytes, s);
+  copy_d2h(valid, dv.p, n, s);
+  stream_sync(s);
+  return count_valid(valid, n);
+}
+void b200_check_points_device(unsigned curve_id, uint8_t* valid, const void* points, uint64_t n) {
+  const Entry entry("b200_check_points_device");
+  check_points_call(curve_id, valid != nullptr && points != nullptr, n);
+  check_points(ctx(), curve_id, valid, points, n);
+}
+void b200_decode_points_device(unsigned curve_id, void* out_p2, uint8_t* valid,
+                               const void* encoded, uint64_t n) {
+  const Entry entry("b200_decode_points_device");
+  check_points_call(curve_id, out_p2 != nullptr && valid != nullptr && encoded != nullptr, n);
+  decode_points(ctx(), curve_id, out_p2, valid, encoded, n);
+}
 unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed) {
   const Entry entry("b200_selftest_lane_arithmetic");
   return selftest_lane_arithmetic(ctx(), warps, seed);

@@ -340,8 +340,14 @@ unsigned field_op_bls12381_gt(const EngineCtx& ctx, unsigned op, uint64_t n, con
                               const uint32_t* b, uint32_t* out);
 unsigned field_op_bn254_gt(const EngineCtx& ctx, unsigned op, uint64_t n, const uint32_t* a,
                            const uint32_t* b, uint32_t* out);
+// square roots (op 27, kOpSqrt of field_op.cuh) in the bls12-381 Fp (field 1) and Fp2 (field 6),
+// in the point-check unit (points.cuh)
+unsigned field_op_sqrt_bls12381(const EngineCtx& ctx, unsigned field, uint64_t n, const uint32_t* a,
+                                uint32_t* out);
 inline unsigned field_op(const EngineCtx& ctx, unsigned field, unsigned op, uint64_t n,
                          const uint32_t* a, const uint32_t* b, uint32_t* out) {
+  if (op == 27)
+    return field == 1 || field == 6 ? field_op_sqrt_bls12381(ctx, field, n, a, out) : ~0u;
   switch (field) {
   case 1: return field_op_bls12381(ctx, op, n, a, b, out);
   case 2: return field_op_bn254(ctx, op, n, a, b, out);
@@ -367,6 +373,35 @@ inline void multi_pairing(const EngineCtx& ctx, unsigned curve_id, void* out,
     multi_pairing_bls12381(ctx, out, num_products, lengths, g1, g2);
   else
     multi_pairing_bn254(ctx, out, num_products, lengths, g1, g2);
+}
+
+// point validation and decoding (points.cuh; the contracts of b200_check_points_device and
+// b200_decode_points_device, curve_id 1-5 checked by the caller): valid[i] = 1 when points[i] (projective
+// ABI structs) / encoded[i] (commitments) is a point of the order-r group; decoded points go to out_p2
+void check_points_bls12381(const EngineCtx& ctx, unsigned curve_id, uint8_t* valid,
+                           const void* points, uint64_t n);
+void check_points_bn254(const EngineCtx& ctx, unsigned curve_id, uint8_t* valid, const void* points,
+                        uint64_t n);
+void decode_points_bls12381(const EngineCtx& ctx, unsigned curve_id, void* out_p2, uint8_t* valid,
+                            const void* encoded, uint64_t n);
+void decode_points_bn254(const EngineCtx& ctx, unsigned curve_id, void* out_p2, uint8_t* valid,
+                         const void* encoded, uint64_t n);
+inline bool points_bls12381(unsigned curve_id) {
+  return curve_id == SXT_CURVE_BLS_381 || curve_id == B200_CURVE_BLS12_381_G2;
+}
+inline void check_points(const EngineCtx& ctx, unsigned curve_id, uint8_t* valid,
+                         const void* points, uint64_t n) {
+  if (points_bls12381(curve_id))
+    check_points_bls12381(ctx, curve_id, valid, points, n);
+  else
+    check_points_bn254(ctx, curve_id, valid, points, n);
+}
+inline void decode_points(const EngineCtx& ctx, unsigned curve_id, void* out_p2, uint8_t* valid,
+                          const void* encoded, uint64_t n) {
+  if (points_bls12381(curve_id))
+    decode_points_bls12381(ctx, curve_id, out_p2, valid, encoded, n);
+  else
+    decode_points_bn254(ctx, curve_id, out_p2, valid, encoded, n);
 }
 
 // built-in ristretto generators g(first .. first+n) into the device generator layout

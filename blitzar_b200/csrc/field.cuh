@@ -1035,6 +1035,17 @@ template <class B, class P> struct Fp2 {
   static B200_HD void invert(E& r, const E& a) { invert_by_norm<false>(r, a); }
   static B200_HD void invert_eea(E& r, const E& a) { invert_by_norm<true>(r, a); }
 
+  // a^e for a public exponent of H limbs (as Mont::pow)
+  template <class C> static B200_HD void pow(E& r, const E& a, C expo) {
+    E acc = one();
+    for (int i = 32 * H - 1; i >= 0; --i) {
+      sqr(acc, acc);
+      if ((expo(i >> 5) >> (i & 31)) & 1u)
+        mul(acc, acc, a);
+    }
+    r = acc;
+  }
+
   static B200_HD void from_mont(E& r, const E& a) {
     Be c0, c1;
     B::from_mont(c0, part(a, 0));

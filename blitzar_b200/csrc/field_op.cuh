@@ -19,6 +19,7 @@ enum : u32 {
   kOpInvertEea, kOpFromMont, kOpToMont, kOpLexLargest,               // Montgomery fields
   kOpCarry1, kOpSub2p, kOpSub4p, kOpSlice, kOpGather,                // lane-sliced F25519
   kOpFrobenius, kOpCyclotomicSqr, kOpFinalExp,                       // Fp12 (pairing.cuh)
+  kOpSqrt,                                                           // bls12-381 Fp, Fp2 (points.cuh)
 };
 
 // u32 limbs per element of operand a, operand b (0 = unary) and the result; out = 0: not offered

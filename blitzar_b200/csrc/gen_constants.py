@@ -11,6 +11,7 @@ choice against RFC 9496's decimal values.
 Limb tables are emitted as `switch` functions so that, after loop unrolling, every use folds to an
 immediate operand (no constant-bank or register traffic).
 """
+import math
 import os
 
 P25519 = 2**255 - 19
@@ -189,6 +190,116 @@ def tower_block(prefix, p, r, n, xi0, x):
     return "\n".join(out)
 
 
+def fp2_ops(p):
+    """(mul, inv, pow) of Fp2 = Fp[u] / (u^2 + 1) on pairs (c0, c1); an Fp element is (c, 0)."""
+    def mul(a, b):
+        return ((a[0] * b[0] - a[1] * b[1]) % p, (a[0] * b[1] + a[1] * b[0]) % p)
+
+    def inv(a):
+        n = pow((a[0] * a[0] + a[1] * a[1]) % p, p - 2, p)
+        return (a[0] * n % p, -a[1] * n % p)
+
+    def pw(a, e):
+        acc = (1, 0)
+        for bit in bin(e)[2:]:
+            acc = mul(acc, acc)
+            if bit == "1":
+                acc = mul(acc, a)
+        return acc
+    return mul, inv, pw
+
+
+def ec_mul(p, k, pt):
+    """[k] pt on y^2 = x^3 + b over Fp2 (affine, None = identity, k of either sign)."""
+    mul, inv, _ = fp2_ops(p)
+
+    def sub(a, b):
+        return ((a[0] - b[0]) % p, (a[1] - b[1]) % p)
+
+    def add(a, b):
+        if a is None or b is None:
+            return b if a is None else a
+        if a[0] == b[0]:
+            if sub((0, 0), a[1]) == b[1]:
+                return None
+            x2 = mul(a[0], a[0])
+            lam = mul((3 * x2[0] % p, 3 * x2[1] % p), inv((2 * a[1][0] % p, 2 * a[1][1] % p)))
+        else:
+            lam = mul(sub(b[1], a[1]), inv(sub(b[0], a[0])))
+        x3 = sub(sub(mul(lam, lam), a[0]), b[0])
+        return (x3, sub(mul(lam, sub(a[0], x3)), a[1]))
+    acc = None
+    for bit in bin(abs(k))[2:]:
+        acc = add(acc, acc)
+        if bit == "1":
+            acc = add(acc, pt)
+    return acc if k >= 0 or acc is None else (acc[0], sub((0, 0), acc[1]))
+
+
+def sextic_twist_order(p, t, r):
+    """#E'(Fp2) of the sextic twist whose order r divides, for a curve over Fp of trace t."""
+    t2 = t * t - 2 * p  # the trace over Fp2
+    f2 = (4 * p * p - t2 * t2) // 3
+    f = math.isqrt(f2)
+    assert f * f == f2
+    orders = [p * p + 1 - s for s in ((t2 + 3 * f) // 2, (t2 - 3 * f) // 2, (-t2 + 3 * f) // 2,
+                                      (-t2 - 3 * f) // 2)]
+    hits = [n for n in orders if n % r == 0]
+    assert len(hits) == 1
+    return hits[0]
+
+
+def points_block():
+    """Constants of the point checks and decoding (points.cuh): the square-root exponents of the
+    bls12-381 Fp ((p + 1) / 4) and Fp2 ((p - 3) / 4), b' = 4 (1 + u) of its G2 for decompression, and
+    the endomorphisms of the subgroup checks. Each eigenvalue relation is asserted on the generator,
+    and every group order h r is asserted odd: the complete RCB16 formulas the checks multiply with
+    then never meet a point of order 2."""
+    p, r, x = BLS_Q, BLS_R, BLS_X
+    mul, inv, pw = fp2_ops(p)
+    assert p % 4 == 3
+    g1 = ((BLS_GX, 0), (BLS_GY, 0))
+    # bls12-381 G1 (Scott 2021): phi(x, y) = (beta x, y) = [-x^2] P on the order-r subgroup
+    beta = pow(2, (p - 1) // 3, p)
+    assert beta != 1 and pow(beta, 3, p) == 1
+    minus_x2 = ec_mul(p, -x * x, g1)
+    assert (mul((beta, 0), g1[0]), g1[1]) == minus_x2
+    assert (mul((beta * beta % p, 0), g1[0]), g1[1]) != minus_x2
+    n1 = p + 1 - (x + 1)
+    assert n1 % r == 0 and n1 % 2 == 1
+    # bls12-381 G2 (M-type twist): psi(x, y) = (conj(x) cx, conj(y) cy) = [x] Q
+    cx = inv(pw((1, 1), (p - 1) // 3))
+    cy = inv(pw((1, 1), (p - 1) // 2))
+    g2 = (BLS2_GX, BLS2_GY)
+
+    def psi(pt, gx, gy):
+        return (mul((pt[0][0], -pt[0][1] % p), gx), mul((pt[1][0], -pt[1][1] % p), gy))
+    assert psi(g2, cx, cy) == ec_mul(p, x, g2)
+    n2 = sextic_twist_order(p, x + 1, r)
+    assert n2 % 2 == 1
+    # bn254 G2 (D-type twist): psi = pi of the Miller loop, xi^((p-1)/3), xi^((p-1)/2), = [6 x^2] Q
+    q = BN254_Q
+    bmul, _, bpw = fp2_ops(q)
+    bx, by = bpw((9, 1), (q - 1) // 3), bpw((9, 1), (q - 1) // 2)
+    bg2 = (BN2_GX, BN2_GY)
+    assert (bmul((bg2[0][0], -bg2[0][1] % q), bx), bmul((bg2[1][0], -bg2[1][1] % q), by)) == \
+        ec_mul(q, 6 * BN_X * BN_X, bg2)
+    n5 = sextic_twist_order(q, 6 * BN_X * BN_X + 1, BN254_R)
+    assert n5 % 2 == 1 and n5 == (2 * q - BN254_R) * BN254_R
+    R = 1 << 384
+
+    def mont2(v):
+        return v[0] * R % p + (v[1] * R % p << 384)
+    return "\n".join([
+        "// ---- point checks and decoding (points.cuh)",
+        table("BLS_SQRT_EXP", (p + 1) // 4, 12),   # Fp square root candidate a^((p+1)/4)
+        table("BLS2_SQRT_EXP", (p - 3) // 4, 12),  # Fp2 square root (Adj-Rodriguez-Henriquez alg. 9)
+        table("BLS_BETA", beta * R % p, 12),        # cube root of unity of phi on G1, Montgomery
+        table("BLS2_B", mont2((4, 4)), 24),         # b' = 4 (1 + u)
+        table("BLS2_PSI_X", mont2(cx), 24),         # (1 + u)^(-(p-1)/3)
+        table("BLS2_PSI_Y", mont2(cy), 24)])        # (1 + u)^(-(p-1)/2)
+
+
 L25519 = 2**252 + 27742317777372353535851937790883648493  # order of the ristretto255 group
 
 
@@ -233,6 +344,7 @@ def main():
     parts.append(scalar_block("SC25", L25519, 8))
     parts.append(tower_block("BLS12", BLS_Q, BLS_R, 12, 1, BLS_X))
     parts.append(tower_block("BN12", BN254_Q, BN254_R, 8, 9, BN_X))
+    parts.append(points_block())
     parts.append("}  // namespace b200")
     here = os.path.dirname(os.path.abspath(__file__))
     path, text = os.path.join(here, "constants.cuh"), "\n".join(parts) + "\n"

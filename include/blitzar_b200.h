@@ -324,14 +324,43 @@ uint32_t b200_curve25519_verify_inner_products(
  * e(P, Q) = f^((p^12 - 1)/r) with exactly this exponent: bls12-381 f = conj(f_{|x|,Q}(P)) (the ate
  * Miller function, x = -0xd201000000010000); bn254 f = f_{6x+2,Q}(P) l_{T,pi(Q)}(P) l_{T+pi(Q),-pi^2(Q)}(P)
  * (optimal ate, x = 0x44e992b44a6909f1, T = [6x+2]Q). Points are not checked to be on their curves or
- * in the order-r subgroups. Aborts for another curve_id, null pointers where there are pairs, and 2^31
- * or more pairs in total. Host pointers; synchronises. */
+ * in the order-r subgroups: check points from outside with b200_check_points / b200_decode_points.
+ * Aborts for another curve_id, null pointers where there are pairs, and 2^31 or more pairs in total.
+ * Host pointers; synchronises. */
 void b200_multi_pairing(unsigned curve_id, void* out, uint32_t num_products,
                         const uint32_t* lengths, const void* g1, const void* g2);
 /* as above, but out, g1 and g2 are DEVICE pointers and lengths is a host array; enqueued on the
  * library stream, returns without synchronising */
 void b200_multi_pairing_device(unsigned curve_id, void* out, uint32_t num_products,
                                const uint32_t* lengths, const void* g1, const void* g2);
+/* Point validation, for points that come from outside the library (proofs, commitments, setups).
+ * curve_id 1 (bls12-381 G1), 2 (bn254 G1), 3 (Grumpkin), 4 (bls12-381 G2) or 5 (bn254 G2).
+ * valid[i] = 1 when points[i], the curve's projective *_p2 struct, is a point of the order-r group,
+ * else 0: every coordinate (each Fp component of an Fp2) is a Montgomery residue below p (a
+ * coordinate >= p is invalid even when its value mod p would pass); Z = 0 is the identity, which is
+ * valid, whatever X and Y are; otherwise Y^2 Z = X^3 + b Z^3 and, for curves 1, 4 and 5, the point
+ * lies in the order-r subgroup (curves 2 and 3 have prime order). Returns the number of valid points.
+ * Aborts for another curve_id (a ristretto255 encoding is checked by decoding it) and for null
+ * pointers with n > 0; n == 0 returns 0. Host pointers; synchronises. */
+uint64_t b200_check_points(unsigned curve_id, uint8_t* valid, const void* points, uint64_t n);
+/* Decodes n points in the curve's commitment encoding (the layout and stride the commitment calls
+ * write) into *_p2 structs, with valid[i] as above. Curves 1 and 4: the zcash compressed encoding
+ * exactly as the library writes it; 0x80 must be set (no uncompressed form), 0x40 is the identity
+ * with every other bit zero, else x (G2: x.c1 then x.c0, each below p) must have a square x^3 + b and
+ * y is the root whose lexicographic sign matches 0x20. Curves 2, 3 and 5: the affine struct, infinity
+ * 1 the identity, 0 a point whose X and Y are checked, any other value invalid; the padding bytes are
+ * not read. A valid point is written as {x R, y R, R} (Z = Montgomery one), the identity as {0, R, 0},
+ * and an invalid input as that same identity with valid[i] = 0. Returns the number of valid points:
+ * compare it with n, because an invalid point written as the identity would otherwise drop out of a
+ * pairing product unnoticed. Host pointers; synchronises. */
+uint64_t b200_decode_points(unsigned curve_id, void* out_p2, uint8_t* valid, const void* encoded,
+                            uint64_t n);
+/* the same two calls with DEVICE pointers: enqueued on the library stream, no synchronisation, no
+ * return value (count the valid flags, or check them on the device). With BLITZAR_B200_DEVICES=k,
+ * all four calls run on the primary device. */
+void b200_check_points_device(unsigned curve_id, uint8_t* valid, const void* points, uint64_t n);
+void b200_decode_points_device(unsigned curve_id, void* out_p2, uint8_t* valid,
+                               const void* encoded, uint64_t n);
 /* Self-test of the warp-cooperative (lane-sliced) field arithmetic of the tail kernels against the
  * per-thread arithmetic on `warps` warps of pseudo-random and edge-case operands: returns the number
  * of mismatching checks (0 = pass). */
@@ -349,7 +378,8 @@ unsigned b200_selftest_lane_arithmetic(unsigned warps, unsigned seed);
  * 12 from_radix51 (10 limbs in: 5 x u64), 13 to_radix51 (10 limbs out), 14 sqrt_ratio_m1 (a = u,
  * b = v; out: x, then the was-square flag); fields 1-4, 6 and 7: 10 invert, 15 invert_eea,
  * 16 from_mont, 17 to_mont, 18 lexicographically_largest (1 limb out; fields 6 and 7: the zcash rule,
- * c1 decides unless it is 0); field 5: 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p,
+ * c1 decides unless it is 0); fields 1 and 6: 27 sqrt (out: a root, 0 for a non-square, then the
+ * was-square flag); field 5: 0 add, 4 mul, 11 pow22523, 19 carry1, 20 sub2p, 21 sub4p,
  * 22 slice (8 limbs in), 23 gather (8 limbs out). b is read only by binary ops (add, sub, mul,
  * mul_ref, mul_lat, sqrt_ratio_m1, sub2p, sub4p). Host pointers; synchronises. Returns 0, or ~0u when the field does not offer op. */
 unsigned b200_field_op(unsigned field, unsigned op, uint64_t n, const uint32_t* a,
