@@ -724,8 +724,30 @@ static void ge_msm(ge* r, const ge* g, const uint8_t* scalars, u64 n) {
 }
 static unsigned ipa_log2(u64 n) { unsigned k = 0; while ((1ull << k) < n) ++k; return k; }
 
-void oracle_prove_inner_product(uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value, uint8_t* t203,
-                                u64 n, u64 generators_offset, const uint8_t* a_vector, const uint8_t* b_vector) {
+/* Test-only encodings of a 32-byte little-endian s < p: the bytes a prover could emit for the same
+ * decoded point, or for none. ENC_NEGATED writes p - s (odd, |p - s| = s), ENC_PLUS_P the 256-bit
+ * integer s + p, ENC_TOP_BIT s + 2^255 (s to a decoder that drops bit 255), ENC_REPLACE the
+ * caller's 32 bytes. */
+enum { ENC_CANONICAL = 0, ENC_NEGATED = 1, ENC_PLUS_P = 2, ENC_TOP_BIT = 3, ENC_REPLACE = 4 };
+static const uint8_t P25519_BYTES[32] = {0xed, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                         0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                         0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0x7f};
+static void ipa_reencode(uint8_t* s, uint8_t mode, const uint8_t* replacement) {
+  u64 v[4], pw[4];
+  memcpy(v, s, 32); memcpy(pw, P25519_BYTES, 32);
+  if (mode == ENC_NEGATED) mf_subn(v, pw, v, 4);
+  else if (mode == ENC_PLUS_P) mf_addn(v, v, pw, 4);
+  else if (mode == ENC_TOP_BIT) v[3] |= 1ull << 63;
+  else if (mode == ENC_REPLACE) memcpy(v, replacement, 32);
+  memcpy(s, v, 32);
+}
+
+/* modes: NULL, or 2k bytes [L_0 .. L_(k-1) | R_0 .. R_(k-1)]; replacements: 2k * 32 bytes in the same
+ * order, read for ENC_REPLACE; challenges: NULL, or k * 32 bytes for the round challenges x_j. Every
+ * challenge is taken over the bytes emitted. */
+static void prove_inner_product(uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value, uint8_t* t203,
+                                u64 n, u64 generators_offset, const uint8_t* a_vector, const uint8_t* b_vector,
+                                const uint8_t* modes, const uint8_t* replacements, uint8_t* challenges) {
   oracle_init(); sc_init();
   unsigned k = ipa_log2(n); u64 np = 1ull << k;
   ipa_init(t203, n);
@@ -744,7 +766,12 @@ void oracle_prove_inner_product(uint8_t* l_vector, uint8_t* r_vector, uint8_t* a
     ge_msm(&L, G + mid, a, mid); ge_scalarmult(&t, &Q, &c_l); ge_add(&L, &L, &t);
     ge_msm(&R, G, a + 32 * mid, a_hi); ge_scalarmult(&t, &Q, &c_r); ge_add(&R, &R, &t);
     ristretto_encode(l_vector + 32 * round, &L); ristretto_encode(r_vector + 32 * round, &R);
+    if (modes) {
+      ipa_reencode(l_vector + 32 * round, modes[round], replacements + 32 * round);
+      ipa_reencode(r_vector + 32 * round, modes[k + round], replacements + 32 * (k + round));
+    }
     sc x = ipa_challenge(t203, l_vector + 32 * round, r_vector + 32 * round), xi = sc_inv(x);
+    if (challenges) memcpy(challenges + 32 * round, x.v, 32);
     for (u64 i = 0; i < mid; ++i) { /* a' = x a_lo + x^-1 a_hi (zero padded) */
       sc v = sc_mul(x, sc_load(a + 32 * i));
       if (i < a_hi) v = sc_add(v, sc_mul(xi, sc_load(a + 32 * (mid + i))));
@@ -766,13 +793,33 @@ void oracle_prove_inner_product(uint8_t* l_vector, uint8_t* r_vector, uint8_t* a
   memcpy(ap_value, a, 32);
   free(G); free(a); free(b);
 }
+void oracle_prove_inner_product(uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value, uint8_t* t203,
+                                u64 n, u64 generators_offset, const uint8_t* a_vector, const uint8_t* b_vector) {
+  prove_inner_product(l_vector, r_vector, ap_value, t203, n, generators_offset, a_vector, b_vector, NULL,
+                      NULL, NULL);
+}
+void oracle_prove_inner_product_encoded(uint8_t* l_vector, uint8_t* r_vector, uint8_t* ap_value,
+                                        uint8_t* t203, u64 n, u64 generators_offset, const uint8_t* a_vector,
+                                        const uint8_t* b_vector, const uint8_t* modes,
+                                        const uint8_t* replacements, uint8_t* challenges) {
+  prove_inner_product(l_vector, r_vector, ap_value, t203, n, generators_offset, a_vector, b_vector, modes,
+                      replacements, challenges);
+}
 
-/* ristretto255 decoding (RFC 9496 4.3.1; sxt/ristretto/base/byte_conversion.cc:135-) */
-static int ristretto_decode(ge* p, const uint8_t* bytes) {
+/* ristretto255 decoding (RFC 9496 4.3.1; sxt/ristretto/base/byte_conversion.cc:135-). Test-only lax
+ * decoders skip the checks named in the LAX_* bits of `lax`; LAX_MOD_P reads s as the 256-bit integer
+ * mod p instead of from its low 255 bits. */
+enum { LAX_NONE = 0, LAX_CANONICAL = 1, LAX_SIGN = 2, LAX_MOD_P = 4, LAX_T = 8, LAX_Y = 16 };
+static int ristretto_decode_lax(ge* p, const uint8_t* bytes, int lax) {
   fe s, ss, u1, u2, u2sq, v, t, inv_sqrt, den_x, den_y;
   uint8_t back[32];
   fe_frombytes(&s, bytes); fe_tobytes(back, &s);
-  if (memcmp(back, bytes, 32) != 0 || (bytes[0] & 1)) return 0;
+  if ((lax & LAX_MOD_P) && (bytes[31] & 0x80)) { /* 2^255 = 19 */
+    fe nineteen = {{19, 0, 0, 0, 0}};
+    fe_add(&s, &s, &nineteen);
+  }
+  if (!(lax & LAX_CANONICAL) && memcmp(back, bytes, 32) != 0) return 0;
+  if (!(lax & LAX_SIGN) && (bytes[0] & 1)) return 0;
   fe_sq(&ss, &s); fe_sub(&u1, &FE_ONE, &ss); fe_add(&u2, &FE_ONE, &ss); fe_sq(&u2sq, &u2);
   fe_sq(&t, &u1); fe_mul(&t, &t, &FE_D); fe_neg(&v, &t); fe_sub(&v, &v, &u2sq);
   fe_mul(&t, &v, &u2sq);
@@ -780,12 +827,14 @@ static int ristretto_decode(ge* p, const uint8_t* bytes) {
   fe_mul(&den_x, &inv_sqrt, &u2); fe_mul(&den_y, &inv_sqrt, &den_x); fe_mul(&den_y, &den_y, &v);
   fe_mul(&p->X, &s, &den_x); fe_add(&p->X, &p->X, &p->X); fe_abs(&p->X, &p->X);
   fe_mul(&p->Y, &u1, &den_y); p->Z = FE_ONE; fe_mul(&p->T, &p->X, &p->Y);
-  return was_square && !fe_isneg(&p->T) && !fe_iszero(&p->Y);
+  return was_square && ((lax & LAX_T) || !fe_isneg(&p->T)) && ((lax & LAX_Y) || !fe_iszero(&p->Y));
 }
+static int ristretto_decode(ge* p, const uint8_t* bytes) { return ristretto_decode_lax(p, bytes, LAX_NONE); }
 
-int oracle_verify_inner_product(uint8_t* t203, u64 n, u64 generators_offset, const uint8_t* b_vector,
-                                const uint8_t* product, const uint8_t* a_commit160, const uint8_t* l_vector,
-                                const uint8_t* r_vector, const uint8_t* ap_value) {
+int oracle_verify_inner_product_lax(uint8_t* t203, u64 n, u64 generators_offset, const uint8_t* b_vector,
+                                    const uint8_t* product, const uint8_t* a_commit160,
+                                    const uint8_t* l_vector, const uint8_t* r_vector, const uint8_t* ap_value,
+                                    int lax) {
   oracle_init(); sc_init();
   unsigned k = ipa_log2(n); u64 np = 1ull << k;
   ipa_init(t203, n);
@@ -808,7 +857,8 @@ int oracle_verify_inner_product(uint8_t* t203, u64 n, u64 generators_offset, con
   for (unsigned j = 0; j < k; ++j) {
     ge Lp, Rp; sc xi = sc_inv(x[j]);
     sc el = sc_neg(sc_mul(x[j], x[j])), er = sc_neg(sc_mul(xi, xi));
-    ok &= ristretto_decode(&Lp, l_vector + 32 * j); ok &= ristretto_decode(&Rp, r_vector + 32 * j);
+    ok &= ristretto_decode_lax(&Lp, l_vector + 32 * j, lax);
+    ok &= ristretto_decode_lax(&Rp, r_vector + 32 * j, lax);
     if (!ok) break;
     ge_scalarmult(&t, &Lp, &el); ge_add(&expected, &expected, &t);
     ge_scalarmult(&t, &Rp, &er); ge_add(&expected, &expected, &t);
@@ -819,4 +869,10 @@ int oracle_verify_inner_product(uint8_t* t203, u64 n, u64 generators_offset, con
   uint8_t e1[32], e2[32]; ristretto_encode(e1, &expected); ristretto_encode(e2, &commit);
   free(x); free(G); free(g);
   return ok && memcmp(e1, e2, 32) == 0;
+}
+int oracle_verify_inner_product(uint8_t* t203, u64 n, u64 generators_offset, const uint8_t* b_vector,
+                                const uint8_t* product, const uint8_t* a_commit160, const uint8_t* l_vector,
+                                const uint8_t* r_vector, const uint8_t* ap_value) {
+  return oracle_verify_inner_product_lax(t203, n, generators_offset, b_vector, product, a_commit160,
+                                         l_vector, r_vector, ap_value, LAX_NONE);
 }

@@ -122,15 +122,53 @@ def prove_inner_product(transcript, a, b, generators_offset=0):
     return lv[:rounds], rv[:rounds], ap
 
 
+# encodings the test-only prover can emit for L_j / R_j (oracle_prove_inner_product_encoded)
+ENC_CANONICAL, ENC_NEGATED, ENC_PLUS_P, ENC_TOP_BIT, ENC_REPLACE = range(5)
+# checks of RFC 9496 decoding that the test-only lax verifier skips (bits, combined with |): the
+# canonical check, the sign of s, the sign of t, y != 0; LAX_MOD_P reads s as the 256-bit integer
+# mod p instead of from its low 255 bits
+LAX_NONE, LAX_CANONICAL, LAX_SIGN, LAX_MOD_P, LAX_T, LAX_Y = 0, 1, 2, 4, 8, 16
+
+
+def prove_inner_product_encoded(transcript, a, b, generators_offset=0, l_modes=None, r_modes=None,
+                                replacements=None):
+    """The prover, emitting L_j in encoding l_modes[j] and R_j in r_modes[j] (ENC_*; ENC_REPLACE
+    emits replacements[j] / replacements[k + j]) and taking every challenge over the emitted bytes.
+    Returns (l_vector, r_vector, ap_value, the challenges x_j as [k, 32] bytes)."""
+    n = a.shape[0]
+    rounds = max(0, (n - 1).bit_length())
+    lv = np.zeros((max(rounds, 1), 32), dtype=np.uint8)
+    rv = np.zeros((max(rounds, 1), 32), dtype=np.uint8)
+    ap = np.zeros(32, dtype=np.uint8)
+    modes = np.zeros(2 * rounds + 1, dtype=np.uint8)
+    if l_modes is not None:
+        modes[:rounds] = l_modes
+    if r_modes is not None:
+        modes[rounds:2 * rounds] = r_modes
+    rep = np.zeros((2 * rounds + 1, 32), dtype=np.uint8)
+    x = np.zeros((max(rounds, 1), 32), dtype=np.uint8)
+    if replacements is not None:
+        rep[:2 * rounds] = replacements
+    a = np.ascontiguousarray(a, dtype=np.uint8)
+    b = np.ascontiguousarray(b, dtype=np.uint8)
+    lib().oracle_prove_inner_product_encoded(
+        C.c_void_p(lv.ctypes.data), C.c_void_p(rv.ctypes.data), C.c_void_p(ap.ctypes.data),
+        C.c_void_p(transcript.ctypes.data), C.c_uint64(n), C.c_uint64(generators_offset),
+        C.c_void_p(a.ctypes.data), C.c_void_p(b.ctypes.data), C.c_void_p(modes.ctypes.data),
+        C.c_void_p(rep.ctypes.data), C.c_void_p(x.ctypes.data))
+    return lv[:rounds], rv[:rounds], ap, x[:rounds]
+
+
 def verify_inner_product(transcript, b, product, a_commit, l_vector, r_vector, ap_value,
-                         generators_offset=0):
+                         generators_offset=0, lax=LAX_NONE):
     n = b.shape[0]
     b = np.ascontiguousarray(b, dtype=np.uint8)
     lv = np.ascontiguousarray(l_vector if len(l_vector) else np.zeros((1, 32), np.uint8))
     rv = np.ascontiguousarray(r_vector if len(r_vector) else np.zeros((1, 32), np.uint8))
-    lib().oracle_verify_inner_product.restype = C.c_int
-    return int(lib().oracle_verify_inner_product(
+    lib().oracle_verify_inner_product_lax.restype = C.c_int
+    return int(lib().oracle_verify_inner_product_lax(
         C.c_void_p(transcript.ctypes.data), C.c_uint64(n), C.c_uint64(generators_offset),
         C.c_void_p(b.ctypes.data), C.c_void_p(np.ascontiguousarray(product).ctypes.data),
         C.c_void_p(np.ascontiguousarray(a_commit).ctypes.data), C.c_void_p(lv.ctypes.data),
-        C.c_void_p(rv.ctypes.data), C.c_void_p(np.ascontiguousarray(ap_value).ctypes.data)))
+        C.c_void_p(rv.ctypes.data), C.c_void_p(np.ascontiguousarray(ap_value).ctypes.data),
+        C.c_int(lax)))
