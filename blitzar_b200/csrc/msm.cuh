@@ -311,7 +311,7 @@ inline void exclusive_scan(u32* data, u64 n, stream_t s, u32 chunk = kScanChunkF
 //   4. BinSortBody: per bin, counting sort by key in shared memory, final positions bin start + local
 //      offset, and the bins' bucket end offsets. A bin above kBinCap entries (one micro-bin holding a
 //      very dense bucket) is sorted the same way out of global memory.
-constexpr u32 kMicroBins = 16384, kBinCap = 8192, kBinSpan = 4096, kMaxBinShift = 12;
+constexpr u32 kMicroBins = 16384, kBinCap = 16384, kBinSpan = 4096, kMaxBinShift = 12;
 // below this many entries the atomic path's fewer launches win (MsmOptions::sort_path = 1)
 constexpr u64 kBinnedSortMinEntries = 1ull << 20;
 
@@ -485,9 +485,13 @@ struct CoarseScatterBody {
   }
 };
 
+// A bin's entries are read twice from the temporary array, for the histogram and for the placement;
+// the second read finds them in L2. Only the ordered bin is held in shared memory, so a bin can hold
+// kBinCap = 16384 entries in 144 KB: twice the entries of a copy-then-order layout, so half as many
+// bins for the coarse scatter to count, scan and reserve per tile, and runs per bin twice as long.
 struct BinSortBody {
   static constexpr int kBlock = 1024;
-  static constexpr size_t kSmem = 2 * kBinCap * sizeof(u64) + kBinSpan * sizeof(u32);
+  static constexpr size_t kSmem = kBinCap * sizeof(u64) + kBinSpan * sizeof(u32);
   const u64* tmp;
   const u32* bin_start;
   const u32* bin_micro;
@@ -500,24 +504,18 @@ struct BinSortBody {
     __shared__ u32 ws[32];
     if (b >= *nbins_ptr)
       return;
-    u64* ent = (u64*)smem;
-    u32* h = (u32*)(smem + 2 * kBinCap * sizeof(u64));
+    u64* sorted = (u64*)smem;
+    u32* h = (u32*)(smem + kBinCap * sizeof(u64));
     const u32 lo = bin_start[b], size = bin_start[b + 1] - lo;
     const u64 klo = (u64)bin_micro[b] << shift, khi_m = (u64)bin_micro[b + 1] << shift;
     const u32 span = (u32)((khi_m < nkeys ? khi_m : nkeys) - klo);
-    const bool local = size <= kBinCap;  // else: a dense micro-bin, sorted out of global memory
+    const bool local = size <= kBinCap;  // else: a dense micro-bin, placed straight into global memory
     for (u32 k = threadIdx.x; k < span; k += kBlock)
       h[k] = 0;
-    if (local) {  // plain copy first: the loads stay independent of the histogram atomics
-#pragma unroll 4
-      for (u32 i = threadIdx.x; i < size; i += kBlock)
-        ent[i] = tmp[(u64)lo + i];
-    }
     __syncthreads();
-    for (u32 i = threadIdx.x; i < size; i += kBlock) {
-      const u64 e = local ? ent[i] : tmp[(u64)lo + i];
-      atomicAdd(&h[entry_key(e) - (u32)klo], 1u);
-    }
+#pragma unroll 4
+    for (u32 i = threadIdx.x; i < size; i += kBlock)
+      atomicAdd(&h[entry_key(tmp[(u64)lo + i]) - (u32)klo], 1u);
     __syncthreads();
     const u32 per = (span + kBlock - 1) / kBlock, k0 = min(threadIdx.x * per, span),
               k1 = min(k0 + per, span);
@@ -542,9 +540,9 @@ struct BinSortBody {
     }
     // ordered in shared memory, then written out contiguously: one store per 32 entries of a warp
     // instead of one 32-byte sector per entry
-    u64* sorted = ent + kBinCap;
+#pragma unroll 4
     for (u32 i = threadIdx.x; i < size; i += kBlock) {
-      const u64 e = ent[i];
+      const u64 e = tmp[(u64)lo + i];
       sorted[atomicAdd(&h[entry_key(e) - (u32)klo], 1u)] = e;
     }
     __syncthreads();
@@ -582,11 +580,15 @@ inline void binned_sort(stream_t s, const ColumnDesc* d_cols, const u64* d_col_s
   launch_blocks(PlanBinsBody{micro_counts, nmicro, span_micro, nkeys, bin_of, bin_start, bin_micro,
                              bin_cursor, nbins, counts, d_m},
                 1, nmicro * sizeof(u32), s);
-  // scatter tiles: as many terms as the shared memory left by the two per-bin arrays can stage
+  // scatter tiles: as many terms as the shared memory left by the two per-bin arrays can stage, in
+  // whole rounds of the block's threads (a tile of 1.1 rounds recodes twice in a row on a tenth of
+  // them while the rest wait at the barrier)
   const size_t scatter_smem = 220 * 1024;
   const size_t bin_bytes = (2ull * nmicro + 2) * sizeof(u32);
   const u64 stage_entries = (scatter_smem - bin_bytes) / sizeof(u64);
-  const u64 scatter_tile = std::max<u64>(1, stage_entries / max_windows);
+  u64 scatter_tile = std::max<u64>(1, stage_entries / max_windows);
+  if (scatter_tile > (u64)CoarseScatterBody::kBlock)
+    scatter_tile -= scatter_tile % CoarseScatterBody::kBlock;
   launch_blocks(CoarseScatterBody{d_cols, d_col_start, ncols, c, nbuckets, total_terms,
                                   (u32)scatter_tile, shift, nmicro, bin_of, nbins, bin_cursor, tmp},
                 (total_terms + scatter_tile - 1) / scatter_tile, scatter_smem, s);
@@ -1263,8 +1265,16 @@ struct NormalizeMidBody {
     }
     F::E P, S, total;
     block_prefix_suffix<kBlock>(c, P, S, total, ws);
-    if (threadIdx.x == 0)
-      F::invert(inv_total, total);
+    if (threadIdx.x < 32) {  // 1 / total = total^(p - 2) = (total^(2^252 - 3))^8 * total^3, on 10 lanes
+      const lane10::Lane L = lane10::lane_info();
+      const u32 z = lane10::slice(L, total);
+      const u32 z3 = lane10::mul(L, lane10::mul(L, z, z), z);
+      const u32 r = lane10::mul(L, lane10::sqr_n(L, lane10::pow22523(L, z), 3), z3);
+      F::E inv;
+      lane10::gather(inv, r, 0);
+      if (threadIdx.x == 0)
+        inv_total = inv;
+    }
     __syncthreads();
     F::E inv;  // 1 / c
     F::mul(inv, inv_total, P);
